@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - inference throughput of a BASELINE.json configuration through the fused sm_100a fake-quantization path.
+"""bench.py - inference throughput of a BASELINE.json configuration through the fused sm_90a fake-quantization path.
 
     python bench.py --gpus N --steps K --warmup W            # this framework (one rank per GPU under torchrun)
+    python bench.py ... --dump-outputs DIR                   # + what the last timed step computed, as DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own Python on the box's host CPU cores
 
 Default workload = BASELINE.json configs[2]: ResNet-50 W4A4 (-pcq_w -pcq_a -c laplace -baa -baw -bcw), batch 512 per GPU,
@@ -33,8 +34,8 @@ WORKLOADS = {
     "resnet18_w4a4": (2, "-pcq_w -pcq_a -c laplace -baa -baw -bcw (ResNet-18)"),
 }
 
-# DRAM traffic of the dominant kernel, from profiles/ (bench.py cannot run under ncu itself): ncu dram__bytes_read.sum +
-# dram__bytes_write.sum averaged over the mode-D launches of one step of the named workload.
+# DRAM traffic of the dominant kernel, from profiles/ncu_traffic.json when present (bench.py cannot run under ncu itself):
+# ncu dram__bytes_read.sum + dram__bytes_write.sum averaged over the mode-D launches of one step of the named workload.
 NCU_TRAFFIC_BYTES_PER_LAUNCH = {}
 try:
     with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as _f:
@@ -70,7 +71,11 @@ def parse():
     ap.add_argument("--channels-last", action="store_true", help="accepted for compatibility: this is the default")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the other BASELINE configs, kernel_bench and gpu_baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.channels_last = not args.nchw
     return args
 
@@ -81,7 +86,7 @@ def peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler(object):
@@ -295,6 +300,23 @@ def timed_steps(torch, step, n, barrier):
     return e0.elapsed_time(e1)
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays):
+    """Write each device tensor of `arrays` as `directory`/<name>.npy in float32, at most DUMP_BYTES in all: a larger
+    tensor is cut to a fixed, seeded sample of its rows (same rows in every run with the same arguments)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_BYTES // max(len(arrays), 1)
+    for name, t in sorted(arrays.items()):
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > share:
+            rows = max(share // max(a[:1].nbytes, 1), 1)
+            a = a[np.sort(np.random.RandomState(0).choice(a.shape[0], rows, replace=False))]
+        np.save(os.path.join(directory, name + ".npy"), a)
+
+
 def run_fqb200(args):
     import torch
     import torch.distributed as dist
@@ -312,7 +334,10 @@ def run_fqb200(args):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
     fq._lib.load()
-    torch.backends.cudnn.benchmark = True  # inference_sim.py:205
+    # cuDNN's heuristic algorithm choice, not autotuning (inference_sim.py:205 sets benchmark): autotuning picks by timing,
+    # so another process may pick another convolution algorithm and the same inputs would give other outputs
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
 
     model, qm = pipeline.build_quantized_model(args.config, dev, channels_last=args.channels_last)
     x_host, t_host = pipeline.synthetic_batch(args.batch, seed=1000 + rank, pin=True, channels_last=args.channels_last)
@@ -324,9 +349,14 @@ def run_fqb200(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def step_resident():
         with torch.no_grad():
-            total.add_(pipeline.accuracy_counts(model(x_dev), t_dev))
+            logits = model(x_dev)
+            counts = pipeline.accuracy_counts(logits, t_dev)
+            total.add_(counts)
+        last["logits"], last["accuracy_counts"] = logits, counts
 
     # end to end: every step copies ITS input batch from pinned host memory and reads its 4-float metric vector back.
     # The copy of step k+1 runs on a copy stream while step k computes (double-buffered device staging), which is what
@@ -358,6 +388,8 @@ def run_fqb200(args):
     prof = ops.profile_collect()
     ops.profile_reset(enable=False)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     # ---- timed region 2: end to end from pinned host memory --------------------------------------------
     feeder.start()
@@ -638,7 +670,7 @@ def kernel_bench(torch, dev, peak):
 
 
 def gpu_baseline(torch, dev, peak):
-    """The 'kernel to beat' (BASELINE.md section 3, SURVEY 8c/8d): the reference's own code on the same B200 and tensor
+    """The 'kernel to beat' (BASELINE.md section 3, SURVEY 8c/8d): the reference's own code on the same GPU and tensor
     (512x64x56x56) - its compiled extension incl. the zeros_like / noise tensor of its wrapper, and its pure-PyTorch
     per-channel W4A4 path - next to ours.  Checker code (oracle/_ref) is timed here, never used by the product path."""
     import cnn_quantization_b200 as fq

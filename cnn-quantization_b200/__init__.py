@@ -1,4 +1,4 @@
-"""cnn-quantization_b200: B200-native (sm_100a) implementation of the fake-quantization hot path of
+"""cnn-quantization_b200: H100-native (sm_90a) implementation of the fake-quantization hot path of
 submission2019/cnn-quantization, behind the reference's own ``int_quantization`` / ``IntQuantizer`` API.
 
     from cnn_quantization_b200 import int_quantization          # drop-in for the compiled extension module

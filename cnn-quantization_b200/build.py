@@ -1,8 +1,8 @@
-"""Build the C-ABI shared library ``libfqb200.so`` in-tree with nvcc for sm_100a (no torch headers needed).
+"""Build the C-ABI shared library ``libfqb200.so`` in-tree with nvcc for sm_90a (H100; no torch headers needed).
 
     python cnn-quantization_b200/build.py
 
-The built ``.so`` is git-ignored but travels to the GPU box with the source snapshot.
+The built ``.so`` is git-ignored.
 """
 import os
 import subprocess
@@ -14,10 +14,11 @@ LIB = os.path.join(HERE, "libfqb200.so")
 SOURCES = [os.path.join(CSRC, "fqb200.cu")]
 HEADERS = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [
     os.path.join(os.path.dirname(HERE), "include", "fqb200.h")]
+STAMP = LIB + ".flags"  # the nvcc flags the existing library was built with: one built with other flags is stale
 
 # -fmad=false: the reference's arithmetic is a chain of separately rounded fp32 torch ops; the kernels spell out
 # every fused multiply-add they want (__fmaf_rn) and must not get any other.  No fast-math anywhere.
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 
 
@@ -30,6 +31,12 @@ def nvcc_path():
 
 def is_stale():
     if not os.path.exists(LIB):
+        return True
+    try:
+        with open(STAMP) as f:
+            if f.read().strip() != " ".join(NVCC_FLAGS):
+                return True
+    except OSError:
         return True
     t = os.path.getmtime(LIB)
     return any(os.path.getmtime(p) > t for p in SOURCES + HEADERS)
@@ -46,6 +53,8 @@ def build(force=False, verbose=False):
     if verbose:
         sys.stderr.write(res.stderr)
     os.replace(LIB + ".tmp", LIB)
+    with open(STAMP, "w") as f:
+        f.write(" ".join(NVCC_FLAGS) + "\n")
     return LIB
 
 

@@ -1,8 +1,7 @@
-// fqb200 bulk-copy streaming engine (sm_100a): flat tensors through a ring of shared-memory stages filled by the TMA unit.
+// fqb200 bulk-copy streaming engine (sm_90a): flat tensors through a ring of shared-memory stages filled by the TMA unit.
 //
-// Why (round-2 measurements, profiles/README.md): the per-thread cp.async ring of fq_device.cuh spends ~68 thread
-// instructions per 128-bit vector per phase, most of them cursor / ring bookkeeping, and the phases of L2-resident
-// tensors were issue-bound (5 TB/s from L2).  Here ONE elected thread of a dedicated producer warp issues
+// Why: the per-thread cp.async ring of fq_device.cuh spends most of its thread instructions per 128-bit vector on cursor /
+// ring bookkeeping, and the phases of L2-resident tensors were issue-bound.  Here ONE elected thread of a dedicated producer warp issues
 // `cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes` (1-D TMA, SASS UBLKCP) for a whole 16 KB stage;
 // the 512 consumer threads wait on the stage's `full` mbarrier, read their vectors with LDS.128 and hand the stage back
 // through its `empty` mbarrier (one arrival per consumer warp).  No per-vector address arithmetic, no cp.async groups.
@@ -20,9 +19,9 @@ namespace fqb {
 constexpr int kConsumers = kThreads;             // 512 consumer threads (16 warps)
 constexpr int kBulkThreads = kConsumers + 32;    // + one producer warp
 constexpr int kConsumerWarps = kConsumers / 32;
-// Ring shape (round-2 A/B on the B200, profiles/README.md): ONE CTA per SM with six 32 KB stages beats two CTAs with
-// five 16 KB stages in every phase (S1 of a 411 MB tensor 74.5 vs 85.6 us, 103 MB launch 94 vs 115 us): a bulk request
-// should be large (8 KB stages: 126 us), and 148 CTAs halve the barrier arrivals, atomics and tickets.
+// Ring shape: ONE CTA per SM with six 32 KB stages (192 KB of the 227 KB an H100 block may use).  A bulk request should
+// be large, and one CTA per SM halves the barrier arrivals, atomics and tickets of two.  tools/build_variants.sh builds
+// the other shapes (the macros below) for A/B runs.
 #ifndef FQB_STAGE_VEC
 #define FQB_STAGE_VEC 4
 #endif
@@ -182,7 +181,7 @@ __device__ __forceinline__ void produce_phase(const FlatGeo& g, const float4* sr
     ++k;
     return t < total ? static_cast<unsigned>(t) : 0xffffffffu;
   };
-  // two tickets ahead: the atomic's round trip (~1 us under contention) must not sit in front of a unit's loads
+  // two tickets ahead: the atomic's round trip (long under contention) must not sit in front of a unit's loads
   unsigned cur = fetch();
   unsigned nxt = (cur != 0xffffffffu) ? fetch() : 0xffffffffu;
   while (cur != 0xffffffffu) {

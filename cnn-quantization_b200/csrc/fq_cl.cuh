@@ -11,8 +11,8 @@
 //   S2   read x         sum |x - mean32|  (only when the Laplace b is needed)
 //   A    read x, write  quantize - clip - dequantize
 //
-// No leader sections on the critical path (round-2 stamps: 3.3 us + 16 us per launch, mostly cold instruction fetch of
-// code that ONE CTA ran once): CTAs meet in replicated per-channel accumulators (atomics), a plain grid barrier
+// No leader sections on the critical path (they cost time on every launch, mostly cold instruction fetch of code that
+// ONE CTA ran once): CTAs meet in replicated per-channel accumulators (atomics), a plain grid barrier
 // follows, and then every CTA derives what it needs for ITS channels itself.  The one global computation - bit
 // allocation / mid-tread bin allocation, which needs the std of every channel - runs in CTA 0 while the other CTAs
 // stream phase S2, and is published before CTA 0 arrives at the second barrier.
@@ -64,7 +64,7 @@ __device__ __forceinline__ void red_max_u32(unsigned* p, unsigned v) {
 // Split in two so that a CTA can do useful (instruction-cache warming) work between posting its arrival and waiting.
 // Memory ordering: release / acquire at GPU scope on the arrival counter and the release word (cumulative over the CTA
 // barrier in front), NOT __threadfence(): that is fence.sc.gpu, and a sequentially-consistent fence issued while the other
-// CTAs stream at full bandwidth was measured at ~10 us (round-2 stamps: "aux: iterations" -> "aux solved").
+// CTAs stream at full bandwidth waits for their traffic (debug stamps "aux: iterations" -> "aux solved").
 __device__ __noinline__ void grid_arrive_cl(GridSync* gs, unsigned& epoch) {
   ++epoch;
   consumer_sync();
@@ -100,7 +100,12 @@ __device__ __forceinline__ void grid_exit_cl(GridSync* gs) {
 }
 
 // ---- per-phase accumulators ---------------------------------------------------------------------------------------------
-constexpr unsigned kClChunkStages = (8 + kStageVec - 1) / kStageVec;  // stages (8 vectors) summed in fp32 before folding into float64
+// Stages summed in fp32 before folding into float64: ONE.  A thread reads the same vectors of a stage in the same order
+// whichever CTA consumes it, so a one-stage chunk is a fixed set of elements summed in a fixed order; chunks spanning two
+// stages would pair whatever stages the dynamic work assignment gave a CTA, and the fp32 rounding of the pair (~1e-7)
+// would differ from run to run - enough to move a bit width that sits on its rounding boundary.  What remains
+// order-dependent is the float64 accumulation of the chunks (~1e-16 relative), far below fp32 resolution.
+constexpr unsigned kClChunkStages = 1;
 
 // S1 runs on the RAW values (the bias is a per-channel constant): min / max of x + bias are (min x) + bias and
 // (max x) + bias exactly (rounding is monotone), and mean / std of fl(x + bias) equal mean(x) + bias / std(x) up to the
@@ -379,7 +384,7 @@ struct ClApply {
 // buf: 16 KB of shared memory.  Threads sharing a column (t, t + cv, ...) are reduced by the column's owner items
 // (item it -> column it % cv, channel-in-column it / cv; <= 4 items per thread since 4 * cv <= 2048).  The staging rounds
 // keep their results in registers and ALL the global reductions are issued at the very end: a CTA barrier behind a batch
-// of `red.global` waits for them (round-2 stamps: ~1.8 us per round with the reductions inside the rounds).
+// of `red.global` waits for them (every round would pay that wait with the reductions inside the rounds).
 constexpr unsigned kClItems = 4;
 
 template <typename T, typename Op>
@@ -470,8 +475,8 @@ __device__ __noinline__ void cl_combine_add_f64(unsigned char* buf, unsigned cv,
   }
 }
 
-// sum over the (<= 8) replicas of one accumulator entry: all loads issued before the first add (they are L2 round trips
-// of ~1 us while the other CTAs stream)
+// sum over the (<= 8) replicas of one accumulator entry: all loads issued before the first add (they are slow L2 round
+// trips while the other CTAs stream)
 template <typename T, typename Op>
 __device__ __forceinline__ T cl_rep_reduce(const T* p, unsigned rep, unsigned C, unsigned c, T identity, Op op) {
   T v[8];
@@ -713,7 +718,7 @@ __global__ void __launch_bounds__(kBulkThreads, kBulkCtasPerSm) fq_cl_kernel(con
   // ones only when its consumers are back (it would sit on them otherwise)
   const bool solver_in_s2 = alloc && !aux_needs_b && DEV && gridDim.x > 1u;
   // the producer starts a phase's loads when the consumers are through the previous phase's combine: its reductions
-  // (a few thousand fire-and-forget atomics) queue behind 192 KB of bulk loads otherwise (round-2 stamps: 1.8 us per round)
+  // (a few thousand fire-and-forget atomics) queue behind 192 KB of bulk loads otherwise
   __shared__ alignas(8) unsigned long long phase_go[2];
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(&solver_done), 1u);

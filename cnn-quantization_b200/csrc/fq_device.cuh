@@ -1,4 +1,4 @@
-// fqb200 device-side building blocks (sm_100a).  Header-only, included by fqb200.cu.
+// fqb200 device-side building blocks (sm_90a).  Header-only, included by fqb200.cu.
 //
 // Design notes (see DESIGN.md):
 //  * the hot path is HBM-bound elementwise + reduction work on fp32 NCHW tensors: no tensor cores.
@@ -26,7 +26,7 @@ __device__ __forceinline__ void cta_sync() { asm volatile("bar.sync 1, %0;" ::"n
 // global memory access
 // ------------------------------------------------------------------------------------------------
 // Tensor reads: coherent (the buffer may be written in place later in the same launch), no L1 allocation
-// (each byte is used once per phase; L2 - 126 MB - is what carries reuse between phases).
+// (each byte is used once per phase; L2 - 50 MB on an H100 - is what carries reuse between phases).
 __device__ __forceinline__ float4 ld_tensor(const float4* p) {
   float4 v;
   asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
@@ -213,9 +213,9 @@ __device__ __forceinline__ void grid_exit(GridSync* gs) {
 // The vectors of every group are enumerated in (outer, inner) order: v in [0, group_v).  A work UNIT is the p-th
 // 1/P share of one group: unit u = p * G + g covers v in [group_v*p/P, group_v*(p+1)/P) of group g.  Units are
 // statically defined (so every partial result is reproducible bit for bit) but DYNAMICALLY assigned: CTAs pull the
-// next unit id from an atomic counter.  Measured on B200: with equal static shares the CTAs of a bandwidth-bound
-// phase finish anywhere between 0.65x and 1.3x of the mean (memory arbitration is not fair), and the tail runs at
-// a fraction of the HBM bandwidth; pulling small units instead ends every phase within one unit time.
+// next unit id from an atomic counter.  With equal static shares the CTAs of a bandwidth-bound phase finish at
+// visibly different times (memory arbitration is not fair), and the tail runs at a fraction of the HBM bandwidth;
+// pulling small units instead ends every phase within one unit time.
 // Consecutive ids are neighbouring channels of the same batch slab, so what the CTAs touch concurrently is a
 // nearly contiguous window of memory.  Every unit leaves one partial at slot u.
 //

@@ -1,4 +1,4 @@
-// fqb200: fused fake-quantization kernels for B200 (sm_100a) + the C ABI of include/fqb200.h.
+// fqb200: fused fake-quantization kernels for H100 (sm_90a) + the C ABI of include/fqb200.h.
 //
 // One hooked tensor = one launch of fq_fused_kernel, a persistent cooperative kernel:
 //
@@ -96,8 +96,8 @@ struct FusedArgs {
   // the workspace, right after the barrier words)
   unsigned *amin_inv, *amax;            // max of ~enc(x) (= min) and of enc(x), enc = order-preserving uint encoding
   double *asum, *aabs, *asq;
-  unsigned nhwc_rep;                    // replicas of the accumulators (CTA b adds into replica b % nhwc_rep): 296
-                                        // same-address atomics serialise in L2 (~7 us), 37 do not; rep * C <= 4096
+  unsigned nhwc_rep;                    // replicas of the accumulators (CTA b adds into replica b % nhwc_rep): one
+                                        // address per channel for the whole grid serialises in L2; rep * C <= 4096
 };
 
 constexpr unsigned kMaxNhwcChannels = 4096;
@@ -1177,9 +1177,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 }
 
 // Max pooling on channels-last memory ([N][H][W][C], C % 4 == 0): the operator in front of the `activation_pooling`
-// quantization call site (MaxPool2dWithId.forward, inference_quantization_manager.py:58-74).  torch's NHWC kernel runs at
-// ~1.8 TB/s on the 1.6 GB ResNet stem activation (5 % of a step, 17 % of a VGG-16 step, profiles/README.md round 2); this
-// one is a plain gather of k*k 128-bit vectors per output vector - neighbouring windows overlap in L1 / L2 - with torch's
+// quantization call site (MaxPool2dWithId.forward, inference_quantization_manager.py:58-74), in place of torch's NHWC
+// kernel; this one is a plain gather of k*k 128-bit vectors per output vector - neighbouring windows overlap in L1 / L2 - with torch's
 // NaN rule (a NaN in the window wins).  Results are bit-identical (max is exact).
 struct PoolArgs {
   const float* in;
@@ -1273,6 +1272,7 @@ struct DeviceInfo {
   int resident_rows = 0;        // fq_rows_kernel
 };
 constexpr int kMaxDevices = 64;
+constexpr int kAssumedSms = 132;  // H100 SXM: the SM count plans assume when no device is present
 DeviceInfo g_dev[kMaxDevices];
 std::once_flag g_dev_once[kMaxDevices];
 
@@ -1463,7 +1463,7 @@ struct Plan {
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-constexpr uint64_t kUnitsPerCta = 8;  // dynamic work units per resident CTA (flat above 8: profiles/README.md, round 1)
+constexpr uint64_t kUnitsPerCta = 8;  // dynamic work units per resident CTA
 
 // Choose the access mode (128-bit, bundled 128-bit, scalar), the number of parts per group (unit size) and the grid
 // size; fill the geometry.
@@ -1720,7 +1720,7 @@ size_t fqb200_workspace_bytes(const fqb200_desc* d) {
   if (check_desc(d) != FQB200_OK) return 0;
   if (d->outer <= 0 || d->groups <= 0 || d->inner <= 0) return 256;
   if (d->range_mode == FQB200_RANGE_GIVEN) return 256;  // not used by the launch; non-zero = "descriptor accepted"
-  int resident = 148 * fqb::kCtasPerSm;  // without a device (build container) assume a B200
+  int resident = kAssumedSms * fqb::kCtasPerSm;  // without a device: plan for an H100
   DeviceInfo* di = nullptr;
   if (get_device(&di) == FQB200_OK) resident = di->resident;
   if (d->channels_last) return carve(nullptr, 0, static_cast<uint64_t>(d->groups), nullptr);
@@ -1748,7 +1748,7 @@ int fqb200_plan_info(const fqb200_desc* d, int64_t* out8) {
   if (rc != FQB200_OK) return rc;
   if (!out8) return fail(FQB200_ERR_INVALID, "null output%s");
   DeviceInfo* di = nullptr;
-  int resident = 148 * fqb::kCtasPerSm, resident_cl = 148 * fqb::kCtasPerSm;
+  int resident = kAssumedSms * fqb::kCtasPerSm, resident_cl = kAssumedSms * fqb::kCtasPerSm;
   if (get_device(&di) == FQB200_OK) {
     resident = di->resident;
     resident_cl = di->resident_cl[d->out_hist ? 1 : 0];
@@ -2082,8 +2082,7 @@ int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* worksp
     A.nhwc_rep = r < 1u ? 1u : (r > 8u ? 8u : r);
     A.need_dev = cl_needs_b(d) ? 1 : 0;
     const bool hist = d->out_hist != nullptr;
-    // (A/B on the GPU, profiles/README.md round 2: an ordinary launch of the same grid is not faster; the cooperative one
-    // guarantees the co-residency the grid barriers need)
+    // (the cooperative launch guarantees the co-residency the grid barriers need)
     e = cudaLaunchCooperativeKernel(cl_kernel_ptr(d->leaf, A.need_dev != 0, hist), dim3(pl.grid), dim3(fqb::kBulkThreads), args,
                                     cl_smem(hist), st);
     if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_cl_kernel: %s", cudaGetErrorString(e));

@@ -1,6 +1,6 @@
 """Drop-in ``IntQuantizer`` for the reference's
 ``pytorch_quantizer/quantization/qtypes/int_quantizer.py`` (same constructor dict, same ``__call__``,
-same mutable attributes, same method names), routed to the fused sm_100a kernels in ``libfqb200.so``.
+same mutable attributes, same method names), routed to the fused sm_90a kernels in ``libfqb200.so``.
 
 Where the reference runs ~10 elementwise kernels, several reductions, up to 6 transposed copies and O(C)
 host synchronisations per hooked tensor, every dispatch target below is ONE kernel launch on the tensor's own

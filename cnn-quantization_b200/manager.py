@@ -6,7 +6,7 @@ call sites, same ``quantize_instant`` / ``quantize_model`` semantics, but
   nn.BatchNorm2d`` modules instead of the reference's class swap (``nn.Conv2d = Conv2dWithId`` ..., :518-533).
   While the manager is enabled the stock classes' ``__init__`` is wrapped only to stamp the construction-order
   id the reference's ``*WithId`` counters would have produced (:29,51,77,153,221,255);
-* the quantizers are this package's ``IntQuantizer`` (one fused sm_100a launch per hooked tensor), and the
+* the quantizers are this package's ``IntQuantizer`` (one fused sm_90a launch per hooked tensor), and the
   weight bias / variance correction of ``quantize_model`` (:374-391) happens inside the weight's launch;
 * nothing is a process-wide singleton: several managers can exist (one per rank / model).
 

@@ -1,5 +1,5 @@
 /*
- * fqb200 - B200-native (sm_100a) fake-quantization library: C ABI.
+ * fqb200 - H100-native (sm_90a) fake-quantization library: C ABI.
  *
  * Drop-in boundary for the fake-quantization hot path of submission2019/cnn-quantization
  * (SURVEY.md section 8).  Plain C: device pointers, sizes, a stream handle; no torch types.
@@ -164,7 +164,7 @@ typedef struct fqb200_desc {
 int fqb200_abi_version(void);
 /* text of the last error on the calling thread ("" if none) */
 const char* fqb200_last_error(void);
-/* number of CTAs the fused kernel keeps resident on the current device (148 SMs x 2 on a B200) */
+/* number of CTAs the fused kernel keeps resident on the current device (132 SMs x 2 on an H100) */
 int fqb200_resident_ctas(void);
 
 /* What a launch of `d` would look like on the current device (introspection for tools and tests), 8 values:

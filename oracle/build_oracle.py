@@ -1,13 +1,13 @@
 """Build the test-infrastructure binaries under oracle/ (never loaded by the product):
 
   oracle/_build/liboracle_leaf.so   gcc build of oracle/fq_leaf.c (plain-C leaf restatement, OpenMP)
-  oracle/_ref/int_quantization*.so  the REFERENCE's own extension (kernels/int_quantization.cpp + gemmlowp.cu),
-                                    compiled unmodified for sm_100a from where the sources lie under
-                                    /root/reference - only when that directory exists (build container).
+  oracle/_ref/sm_90a/int_quantization*.so  the REFERENCE's own extension (kernels/int_quantization.cpp + gemmlowp.cu),
+                                    compiled unmodified for sm_90a from where the sources lie under
+                                    REF_ROOT - only when that directory exists.
                                     It is the on-GPU oracle for the compiled leaf and the "kernel to beat".
   oracle/_ref/pyref/                the REFERENCE's Python hot path (pytorch_quantizer/, utils/), staged unmodified at
-                                    build() time so that it travels to the GPU box with the snapshot (oracle/_ref is
-                                    git-ignored, not gpurun-ignored): the live on-GPU oracle for every row of SURVEY 8a
+                                    build() time so that a GPU machine without the reference can run it (oracle/_ref is
+                                    git-ignored): the live on-GPU oracle for every row of SURVEY 8a
                                     (oracle/ref_live.py imports it next to the compiled extension above).  Nothing of it
                                     is ever committed; the product never imports it.
 """
@@ -36,16 +36,23 @@ def build_leaf(force=False):
     return lib
 
 
+REF_ARCH = "9.0a"                                  # TORCH_CUDA_ARCH_LIST of the reference extension
+REF_EXT_DIR = os.path.join(REFDIR, "sm_90a")       # the extension lives in a directory named for its architecture
+
+
 def build_reference_ext(force=False):
-    """Compile the reference's CUDA extension as is (torch C++ extension, sm_100a).  Returns the .so path or None."""
-    if not os.path.isdir(REF_KERNELS):
-        found = glob.glob(os.path.join(REFDIR, "int_quantization*.so"))
-        return found[0] if found else None
-    found = glob.glob(os.path.join(REFDIR, "int_quantization*.so"))
+    """Compile the reference's CUDA extension as is (torch C++ extension, sm_90a) into oracle/_ref/sm_90a/.  Returns the
+    .so path or None.  Only that directory is ever loaded (oracle/ref_live.py): a binary left elsewhere under oracle/_ref
+    by a build for another architecture is never picked up."""
+    found = glob.glob(os.path.join(REF_EXT_DIR, "int_quantization*.so"))
     if found and not force:
         return found[0]
-    os.makedirs(REFDIR, exist_ok=True)
-    work = os.path.join(REFDIR, "_work")
+    if not os.path.isdir(REF_KERNELS):
+        return None
+    for old in found:
+        os.remove(old)
+    os.makedirs(REF_EXT_DIR, exist_ok=True)
+    work = os.path.join(REF_EXT_DIR, "_work")
     os.makedirs(work, exist_ok=True)
     # setup script lives in OUR tree and points at the reference sources in place (nothing is copied)
     setup_py = os.path.join(work, "setup_ref.py")
@@ -56,14 +63,14 @@ def build_reference_ext(force=False):
             "setup(name='int_quantization', ext_modules=[CUDAExtension('int_quantization', "
             "['%s/int_quantization.cpp', '%s/gemmlowp.cu'])], cmdclass={'build_ext': BuildExtension})\n"
             % (REF_KERNELS, REF_KERNELS))
-    env = dict(os.environ, TORCH_CUDA_ARCH_LIST="10.0a", MAX_JOBS="4")
-    res = subprocess.run([sys.executable, setup_py, "build_ext", "--build-lib", REFDIR, "--build-temp",
+    env = dict(os.environ, TORCH_CUDA_ARCH_LIST=REF_ARCH, MAX_JOBS="4")
+    res = subprocess.run([sys.executable, setup_py, "build_ext", "--build-lib", REF_EXT_DIR, "--build-temp",
                           os.path.join(work, "tmp")], cwd=work, env=env, capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout[-2000:] + res.stderr[-4000:])
         return None
     shutil.rmtree(work, ignore_errors=True)
-    found = glob.glob(os.path.join(REFDIR, "int_quantization*.so"))
+    found = glob.glob(os.path.join(REF_EXT_DIR, "int_quantization*.so"))
     return found[0] if found else None
 
 

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE (like everything under oracle/): the REFERENCE itself as a live oracle on the GPU box.
 
 oracle/build_oracle.py stages the reference's Python packages unmodified under oracle/_ref/pyref and compiles its CUDA
-extension unmodified into oracle/_ref/ (both git-ignored, both travel with the gpurun snapshot).  This module imports
+extension unmodified into oracle/_ref/ (both git-ignored build products of build()).  This module imports
 them so that GPU tests can run ``IntQuantizer`` (int_quantizer.py:56-632) and the reference's own inference manager
 (inference_quantization_manager.py) on the very CUDA tensors our kernels see, at any size.
 
@@ -24,7 +24,8 @@ _state = {}
 
 
 def ext_path():
-    found = glob.glob(os.path.join(REFDIR, "int_quantization*.so"))
+    from oracle.build_oracle import REF_EXT_DIR   # built for this project's GPU architecture, nothing else
+    found = glob.glob(os.path.join(REF_EXT_DIR, "int_quantization*.so"))
     return found[0] if found else None
 
 

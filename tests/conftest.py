@@ -13,7 +13,7 @@ for p in (ROOT, GOLD):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (pytest -m gpu)")
     # the CPU checkers (torch ops, the OpenMP C leaf) must not start more threads than the container's CPU quota:
     # 128 threads under a 16-CPU quota spend their time throttled at barriers
     from oracle.host import host_threads

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Generate the CPU golden fixtures by running the REAL reference (read-only, /root/reference).
+"""Generate the CPU golden fixtures by running the REAL reference (read-only, at REF below).
 
-Run in the build container only (the GPU box has no /root/reference):
+Run only where the reference is checked out (no GPU needed):
 
     python tests/golden/make_golden.py            # writes tests/golden/ref_cpu_*.npz + ref_census.json
 
 The reference has no tests or golden vectors of its own (SURVEY.md section 4), so the fixtures are the
 reference's *outputs*: its pure-PyTorch hot path (int_quantizer.py) executed on CPU tensors with a
 stub `int_quantization` module (the compiled leaf needs a GPU: it is compared live with the reference's own extension
-on the B200, tests/test_gpu_ref_ext.py and tests/test_gpu_ref_live.py).  Inputs are drawn from numpy RandomState (stable across versions) and stored
+on the GPU, tests/test_gpu_ref_ext.py and tests/test_gpu_ref_live.py).  Inputs are drawn from numpy RandomState (stable across versions) and stored
 in the fixture next to the outputs.  Nothing here is imported by the product or by the GPU tests.
 """
 import json

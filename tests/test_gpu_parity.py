@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI / the drop-in Python API) against the CPU oracle and the
+"""GPU parity: the sm_90a kernels (through the C ABI / the drop-in Python API) against the CPU oracle and the
 golden fixtures generated from the real reference.
 
 Two-tier protocol (SURVEY.md section 7, "hard parts"):

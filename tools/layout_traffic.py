@@ -2,8 +2,8 @@
 (diagnostic; round-1 VERDICT item 3 asked for the DRAM bytes of the L2-resident layouts).
 
     ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none \
-        -k regex:fq_cl_kernel --csv --log-file gpurun_out/layout_traffic.csv python tools/layout_traffic.py
-    python tools/layout_traffic.py --summarise gpurun_out/layout_traffic.csv
+        -k regex:fq_cl_kernel --csv --log-file layout_traffic.csv python tools/layout_traffic.py
+    python tools/layout_traffic.py --summarise layout_traffic.csv
 
 Every launch runs on a tensor a 256 MB memset has just pushed out of L2 (the worst case: inside a model step the
 convolution that produced the tensor leaves part of it in L2)."""

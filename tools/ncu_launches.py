@@ -1,6 +1,6 @@
 """Summarise an `ncu --csv` launch list (long format: one row per metric per launch).
 
-    python tools/ncu_launches.py gpurun_out/launches.csv [--traffic-key resnet50_w4a4/512/nhwc]
+    python tools/ncu_launches.py launches.csv [--traffic-key resnet50_w4a4/512/nhwc]
 
 Prints per-kernel launch counts, summed gpu__time_duration and the share of the total; with dram__bytes_* metrics present
 also the DRAM traffic per launch of every fq_* kernel.  --traffic-key writes / updates profiles/ncu_traffic.json with the

@@ -37,5 +37,5 @@ for (n, c, hw) in shapes:
                 best = (tot, buf.cpu().tolist())
         tot, t = best
         gb = n * c * hw * hw * 16 / 1e9
-        print((n, c, hw), "NHWC" if cl else "NCHW", "total %.1f us (%.2f of 6577 GB/s)" % (tot, gb / (tot * 1e-6) / 6577.4),
+        print((n, c, hw), "NHWC" if cl else "NCHW", "total %.1f us (%.2f of the H100 data sheet's 3350 GB/s)" % (tot, gb / (tot * 1e-6) / 3350.0),
               " | ".join("%s %.1f" % (nm, (t[i] - t[0]) / 1e3) for i, nm in order if t[i]))
