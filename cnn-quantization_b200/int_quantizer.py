@@ -103,11 +103,8 @@ class IntQuantizer(object):
         # (columns _lib.STAT_COLUMNS) in ``last_stats`` - what the parity tests compare with the reference's values
         self.export_stats = False
         self.last_stats = None
-        self._relu_follows = False
-        self._bca = None
-        self._residual, self._residual_used = None, False
-        self._defer, self._deferred = False, None
-        self._pool, self._pooled = None, False
+        # per-call inputs of ``__call__``'s extensions (reset when the call returns)
+        self._relu_follows, self._bca, self._residual, self._defer, self._pool = False, None, None, False, None
 
     # ------------------------------------------------------------------------------------------
     # dispatch (int_quantizer.py:92-122)
@@ -143,9 +140,9 @@ class IntQuantizer(object):
             setattr(self, override_att[0], override_att[1])
         self._relu_follows = bool(relu_follows) and self._positive()
         self._bca = bias_correct
-        self._residual, self._residual_used = residual, False
-        self._defer, self._deferred = bool(defer), None
-        self._pool, self._pooled = (tuple(pool) if pool is not None else None), False
+        self._residual = residual
+        self._defer = bool(defer)
+        self._pool = tuple(pool) if pool is not None else None
         try:
             self._unsupported(stat_id)
             if bias is not None and not self._bias_fusable(tensor):
@@ -170,23 +167,12 @@ class IntQuantizer(object):
                     res = self.gemmlowpQuantizeActivationPerChannel(tensor, id, tag, stat_id=stat_id, bias=bias)
             else:
                 res = self.gemmlowpMinMaxQuantize(tensor, tag, stat_id=stat_id, weight_correction=weight_correction, bias=bias)
+            if self._relu_follows and isinstance(res, torch.Tensor):
+                res._fq_nonneg = res._version   # void as soon as somebody modifies the tensor in place
         finally:
             if override_att is not None:
                 setattr(self, override_att[0], orig_att)
-        if self._relu_follows and isinstance(res, torch.Tensor):
-            res._fq_nonneg = res._version   # void as soon as somebody modifies the tensor in place
-        if self._residual_used:
-            res._fq_residual_fused = True
-            res._fq_nonneg = res._version   # the fused epilogue ends with the ReLU
-        if self._deferred is not None:
-            res._fq_deferred = self._deferred
-        if self._pooled:
-            res._fq_pooled = self._pooled   # 2 / 3: which pooling the launch has done
-        self._defer, self._deferred = False, None
-        self._pool, self._pooled = None, False
-        self._relu_follows = False
-        self._bca = None
-        self._residual, self._residual_used = None, False
+            self._relu_follows, self._bca, self._residual, self._defer, self._pool = False, None, None, False, None
         return res
 
     def __repr__(self):
@@ -224,18 +210,8 @@ class IntQuantizer(object):
             return (tensor.shape[2] * tensor.shape[3]) % 4 == 0
         return ops.cl_eligible(tensor)   # channels-last: the bias is a per-thread constant (bias_period = -C)
 
-    @staticmethod
-    def _dense(tensor):
-        return tensor.is_contiguous() or (tensor.dim() == 4 and tensor.is_contiguous(memory_format=torch.channels_last))
-
     def _out(self, tensor):
-        return tensor if (self.inplace and self._dense(tensor)) else None
-
-    @staticmethod
-    def _channels_last(tensor):
-        """An NCHW-shaped activation stored NHWC that the channels-last kernels take as is: C % 4 == 0, C <= 2048 (else it
-        is made NCHW-contiguous first, like every other strided input)."""
-        return ops.cl_eligible(tensor)
+        return tensor if (self.inplace and ops.dense(tensor)) else None
 
     # `-me` (SURVEY.md 8f rank 3): the apply phase histograms the integer grid into 256 counters; the Shannon entropy of
     # utils/entropy.py:6-17 (which runs torch.unique over the whole tensor) is a 256-element computation afterwards
@@ -288,21 +264,21 @@ class IntQuantizer(object):
     def _quantize1(self, tensor, delta, offset, bits=None, layout=None, bias=None):
         """Mode A launch; with ``bias_correct`` set the activation bias correction rides along."""
         if self._bca is None or tensor.dim() != 4:
-            if (self._defer and layout is not None and ops.cl_eligible(tensor, layout) and torch.is_tensor(delta)
-                    and delta.numel() == layout[1] and not self.measure_entropy):
-                # `defer` with known parameters: nothing to launch at all - the call that takes the tensor as its residual
-                # gets the leaf parameters as the table a stats_only launch would have exported (columns 8..11)
-                self._deferred = (self._given_table(delta, offset, bits), bias)
-                return tensor
-            if (layout is not None and (self._residual is not None or self._pool is not None) and ops.cl_eligible(tensor, layout)
-                    and torch.is_tensor(delta) and delta.numel() == layout[1] and not self.measure_entropy):
+            # per-channel parameters of a channels-last tensor that the descriptor entry point takes as it is
+            if ((self._defer or self._residual is not None or self._pool is not None) and layout is not None
+                    and torch.is_tensor(delta) and delta.numel() == layout[1] and not self.measure_entropy
+                    and ops.cl_eligible(tensor, layout)):
+                if self._defer:
+                    # nothing to launch at all: the call that takes the tensor as its residual gets the leaf parameters as
+                    # the table a stats_only launch would have exported (columns 8..11)
+                    tensor._fq_deferred = (self._given_table(delta, offset, bits), bias)
+                    return tensor
                 # the same leaf through the descriptor entry point, which can also finish a ResNet block / pool (`-sm use`)
                 return self._launch(tensor, layout, channels_last=True, range_mode=L.RANGE_GIVEN, leaf=L.LEAF_TORCH,
                                     num_bits=min(self.num_bits, 8), given=(delta, offset, bits), bias=bias, out=self._out(tensor))
             return ops.quantize1(tensor, delta, offset, self.num_bits, bits=bits, layout=layout, bias=bias, out=self._out(tensor))
         relu_first = bool(self._bca)
-        c = tensor.shape[1]
-        if c % 4 == 0 and 4 <= c <= 2048:
+        if ops.cl_channels_ok(tensor.shape[1]):   # else no channels-last copy would qualify either
             x = tensor if ops.cl_eligible(tensor) else tensor.contiguous(memory_format=torch.channels_last)
             if ops.cl_eligible(x):
                 return ops.quantize1_bca(x, delta, offset, self.num_bits, bits=bits, bias=bias, relu_first=relu_first,
@@ -334,13 +310,7 @@ class IntQuantizer(object):
         if (r is None or self.measure_entropy or r.shape != tensor.shape or r.stride() != tensor.stride()
                 or r.dtype != torch.float32 or r.device != tensor.device):
             return {}
-        if rows:
-            n = tensor.shape[0]
-            dense = tensor.is_contiguous() or (tensor.dim() == 4 and tensor.is_contiguous(memory_format=torch.channels_last))
-            if not (dense and tensor.dim() == 4 and n <= 4096 and (tensor.numel() // n) % 4 == 0
-                    and tensor.data_ptr() % 16 == 0 and r.data_ptr() % 16 == 0):
-                return {}
-        elif not channels_last:
+        if not (ops.rows_eligible(tensor, r) if rows else channels_last):
             return {}
         kw = dict(residual=r, residual_relu=True)
         deferred = getattr(r, "_fq_deferred", None)
@@ -349,42 +319,35 @@ class IntQuantizer(object):
             if (rbias is None) != (bias is None) or (rbias is not None and rbias.numel() != bias.numel()) or self.mtd_quant:
                 return {}
             kw.update(residual_stats=stats, residual_bias=rbias)
-        self._residual_used = True
         return kw
 
     def _launch(self, tensor, layout, channels_last=False, rows=False, **kw):
         """One fused launch of the activation paths that can end a ResNet block: deferred (statistics only, see
-        ``__call__``), with the block epilogue (``residual``), or plain."""
-        if self._defer and kw.get("hist") is None and kw.get("range_mode") != L.RANGE_GIVEN and self._can_defer(tensor, channels_last, rows):
+        ``__call__``), pooled, with the block epilogue (``residual``), or plain.  Tags the result with what it did."""
+        if (self._defer and kw.get("hist") is None and kw.get("range_mode") != L.RANGE_GIVEN and not self.measure_entropy
+                and not self.mtd_quant and tensor.dtype == torch.float32 and (ops.rows_eligible(tensor) if rows else channels_last)):
             skw = {k: v for k, v in kw.items() if k not in ("out", "hist")}
             stats = ops.fused(tensor, layout, stats_only=True, channels_last=channels_last, **skw)
             if self.export_stats:
                 self.last_stats = stats
-            self._deferred = (stats, kw.get("bias"))
+            tensor._fq_deferred = (stats, kw.get("bias"))
             return tensor
         # (a ReLU between quantizer and pooling must be one the caller is going to skip: it has to hand the SAME tensor on)
-        if (self._pool is not None and self._pool[:2] in ((2, 2), (3, 3)) and (self._relu_follows or self._pool[2:] == ("direct",))
-                and ((channels_last and not rows) or (rows and kw.get("bias") is not None and kw.get("bias_period", 0) < 0
-                                                      and tensor.dim() == 4 and not tensor.is_contiguous()
-                                                      and tensor.is_contiguous(memory_format=torch.channels_last)
-                                                      and tensor.shape[1] % 4 == 0 and tensor.shape[1] <= 2048))
-                and kw.get("hist") is None and self._residual is None and not self._defer
-                and tensor.dim() == 4 and tensor.shape[2] >= 2 and tensor.shape[3] >= 2 and tensor.shape[3] % 2 == 0
-                and (self._pool[0] == 2 or (tensor.shape[2] % 2 == 0 and tensor.shape[1] <= 896))):   # 3x3: 9 * C/4 vectors per stage
-            kw.pop("out", None)   # only the pooled tensor is written
-            self._pooled = self._pool[0]
-            return self._fused(tensor, layout, channels_last=channels_last, pool=self._pool[:2], **kw)
-        return self._fused(tensor, layout, channels_last=channels_last, **kw,
-                           **self._residual_kw(tensor, channels_last, rows=rows, bias=kw.get("bias")))
-
-    def _can_defer(self, tensor, channels_last, rows):
-        if self.measure_entropy or self.mtd_quant or tensor.dim() != 4 or tensor.dtype != torch.float32:
-            return False
-        if rows:
-            n = tensor.shape[0]
-            dense = tensor.is_contiguous() or tensor.is_contiguous(memory_format=torch.channels_last)
-            return dense and n <= 4096 and (tensor.numel() // n) % 4 == 0 and tensor.data_ptr() % 16 == 0
-        return bool(channels_last)
+        pool = self._pool
+        if pool is not None and (self._relu_follows or pool[2:] == ("direct",)) and not self._defer:
+            rows_cl = rows and kw.get("bias_period", 0) < 0 and ops.cl_eligible(tensor)   # C from the channel-fastest bias
+            if (ops.pool_request_ok(tensor, pool[:2], channels_last or rows_cl, residual=self._residual, hist=kw.get("hist"))
+                    and ops.pool_tile_fits(tensor, pool[0])):
+                kw.pop("out", None)   # only the pooled tensor is written
+                res = self._fused(tensor, layout, channels_last=channels_last, pool=pool[:2], **kw)
+                res._fq_pooled = pool[0]   # 2 / 3: which pooling the launch has done
+                return res
+        rkw = self._residual_kw(tensor, channels_last, rows=rows, bias=kw.get("bias"))
+        res = self._fused(tensor, layout, channels_last=channels_last, **kw, **rkw)
+        if rkw:
+            res._fq_residual_fused = True
+            res._fq_nonneg = res._version   # the fused epilogue ends with the ReLU
+        return res
 
     def _fused(self, tensor, layout, **kw):
         """ops.fused, keeping the exported statistics table when ``export_stats`` is set."""
@@ -478,7 +441,7 @@ class IntQuantizer(object):
         mode, k = self._range_mode(clip_type)
         if self._pc_act(tensor) and tensor.shape[1] > 1:
             hist = self._hist(tensor)  # the reference measures entropy in gemmlowpQuantizeActivationPerChannel (:442-445)
-            res = self._launch(tensor, self._nchw_layout(tensor), channels_last=self._channels_last(tensor),
+            res = self._launch(tensor, self._nchw_layout(tensor), channels_last=ops.cl_eligible(tensor),
                                scope=L.SCOPE_GROUP, range_mode=mode, clip_k=k,
                                leaf=L.LEAF_TORCH, num_bits=self.num_bits, positive=self._positive(),
                                bit_alloc=self.bit_alloc_act, bit_alloc_prior=self._prior(),
@@ -557,7 +520,7 @@ class IntQuantizer(object):
             return self._quantize1(tensor, delta, offset, bits=bits, layout=layout, bias=bias)
         if min_ is None and max_ is None:
             hist = self._hist(tensor)
-            res = self._launch(tensor, layout, channels_last=self._channels_last(tensor),
+            res = self._launch(tensor, layout, channels_last=ops.cl_eligible(tensor),
                                scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.LEAF_TORCH,
                                num_bits=self.num_bits, positive=self._positive(), bit_alloc=self.bit_alloc_act,
                                bit_alloc_prior=self._prior(), bit_alloc_round=self.bit_alloc_round,
@@ -674,7 +637,7 @@ class IntQuantizer(object):
     def mid_tread_quantize_activation_per_channel(self, tensor, id, bias=None):
         layout = self._nchw_layout(tensor)
         kw = dict(leaf=L.LEAF_MIDTREAD, positive=self._positive(), mt_target=self.bit_alloc_target_act, mt_clip=True, bias=bias,
-                  out=self._out(tensor), channels_last=self._channels_last(tensor))
+                  out=self._out(tensor), channels_last=ops.cl_eligible(tensor))
         if not self.measure_entropy:
             return self._launch(tensor, layout, **kw)   # the mid-tread leaf is monotone too: block epilogue / pooling apply
         if kw["channels_last"]:

@@ -169,9 +169,8 @@ def _maxpool_forward(pool):
             return x   # the quantization launch of the convolution in front has pooled already (IntQuantizer ``pool``)
         if pending:
             raise RuntimeError("a tensor pooled inside its quantization launch lost its tag on the way to %r" % (pool,))
-        if (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and not x.requires_grad and not pool.return_indices
-                and not pool.ceil_mode and pool.dilation in (1, (1, 1)) and x.shape[1] % 4 == 0 and not x.is_contiguous()
-                and x.is_contiguous(memory_format=torch.channels_last)):
+        if (x.is_cuda and x.dtype == torch.float32 and not x.requires_grad and not pool.return_indices
+                and not pool.ceil_mode and pool.dilation in (1, (1, 1)) and ops.nhwc(x) and x.shape[1] % 4 == 0):
             stride = pool.stride if pool.stride is not None else pool.kernel_size
             return ops.maxpool2d_cl(x, pool.kernel_size, stride, pool.padding)
         return orig(pool, x)
@@ -198,7 +197,7 @@ def _residual_block_forward(block, bottleneck, manager):
         # max(quantize(conv) + identity, 0) - in its apply phase, when the folded BN behind the convolution is the
         # identity.  The set of quantize_instant calls is unchanged; the shortcut's call moves one position forward.
         early = (manager.fuse_residual_into_quant and manager.enabled and manager.bn_folding and hasattr(last_bn, "absorbed")
-                 and x.is_cuda and x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last))
+                 and x.is_cuda and ops.nhwc(x))
         if early:
             if block.downsample is not None:
                 # ... and the shortcut convolution's output is used by that launch only: its own launch can stop after
@@ -225,7 +224,7 @@ def _residual_block_forward(block, bottleneck, manager):
         if not early and block.downsample is not None:
             identity = block.downsample(x)
         if (out.is_cuda and out.dtype == torch.float32 and identity.dtype == torch.float32 and out.shape == identity.shape
-                and out.stride() == identity.stride() and ops._dense(out) and not out.requires_grad):
+                and out.stride() == identity.stride() and ops.dense(out) and not out.requires_grad):
             return ops.add_relu_(out, identity)
         out += identity
         return block.relu(out)

@@ -78,19 +78,55 @@ def _workspace(device, stream, nbytes):
     return ws
 
 
-def _dense(t):
-    return t.is_contiguous() or (t.dim() == 4 and t.is_contiguous(memory_format=torch.channels_last))
+def nhwc(x):
+    """True when ``x`` is 4-D and stored channels-last without also being NCHW-contiguous (C == 1, H == W == 1)."""
+    return x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
+
+
+def dense(t):
+    return t.is_contiguous() or nhwc(t)
+
+
+def cl_channels_ok(c):
+    """Channel counts the channels-last kernels take (flat_eligible in fqb200.cu)."""
+    return c % 4 == 0 and 4 <= c <= 2048
 
 
 def cl_eligible(x, layout=None):
     """True when ``x`` is an NCHW-shaped activation stored channels-last that the flat-stream kernels take as it is:
-    C % 4 == 0, C <= 2048 (``layout``, when given, must be its (N, C, H*W) view)."""
-    if x.dim() != 4 or x.is_contiguous() or not x.is_contiguous(memory_format=torch.channels_last):
+    C % 4 == 0, C <= 2048, 16-byte aligned (``layout``, when given, must be its (N, C, H*W) view)."""
+    if not nhwc(x):
         return False
     n, c = x.shape[0], x.shape[1]
     if layout is not None and tuple(int(v) for v in layout) != (n, c, x.numel() // (n * c)):
         return False
-    return c % 4 == 0 and 4 <= c <= 2048 and x.data_ptr() % 16 == 0
+    return cl_channels_ok(c) and x.data_ptr() % 16 == 0
+
+
+def rows_eligible(x, other=None):
+    """True when the per-sample / per-tensor min-max kernel takes the 4-D ``x`` (and ``other``, an operand read alongside)
+    as it is: dense, N <= 4096 samples of a multiple of 4 elements, 16-byte aligned (rows_supported in fqb200.cu)."""
+    if x.dim() != 4 or not dense(x):
+        return False
+    n = x.shape[0]
+    return n <= 4096 and (x.numel() // n) % 4 == 0 and x.data_ptr() % 16 == 0 and (other is None or other.data_ptr() % 16 == 0)
+
+
+# 3x3 pooling: one tile reads three input rows of at least 3 pixels, 9 * C/4 vectors, from one ring stage.  This mirrors
+# the tile-width search of fqb200_fused, which would take a few channels more (C <= 908 with the default stage size).
+POOL3_MAX_CHANNELS = 896
+
+
+def pool_request_ok(x, pool, nhwc_launch, stats_only=False, residual=None, hist=None):
+    """True when ``fused`` accepts ``pool``: (2, 2) or (3, 3) on a launch that reads channels-last memory (``nhwc_launch``: a
+    channels_last launch, or a rows launch told C by a channel-fastest bias), no residual / histogram, W even (3x3: H too)."""
+    return (tuple(pool) in ((2, 2), (3, 3)) and nhwc_launch and not stats_only and residual is None and hist is None
+            and x.shape[3] % 2 == 0 and (pool[0] == 2 or x.shape[2] % 2 == 0))
+
+
+def pool_tile_fits(x, kind):
+    """True when the library finds a pooling tile for the channels-last [N, C, H, W] ``x`` (``kind`` 2 or 3)."""
+    return x.shape[2] >= 2 and x.shape[3] >= 2 and (kind == 2 or x.shape[1] <= POOL3_MAX_CHANNELS)
 
 
 def _resolve_out(x, out):
@@ -129,7 +165,7 @@ def float2gemmlowp(x, range_, offset, num_bits, int_exp, enforce_true_zero, nois
         if noise.shape != x.shape:
             raise ValueError("noise must have the shape of the input")
     # one parameter set for the whole tensor: any dense memory order will do (no copy for channels-last activations)
-    if not _dense(x) or (noise is not None and noise.stride() != x.stride()):
+    if not dense(x) or (noise is not None and noise.stride() != x.stride()):
         x = x.contiguous()
         noise = noise.contiguous() if noise is not None else None
     kout, uout = _resolve_out(x, out)
@@ -152,7 +188,7 @@ def quantize1(x, delta, offset, num_bits, bits=None, layout=None, want_grid=Fals
     # channels-last activations with per-channel parameters run on the NHWC memory as it is (layout = (N, C, H*W));
     # one parameter set for the whole tensor does not care about the memory order at all
     cl = bool(per_group and layout is not None and cl_eligible(x, layout))
-    if not cl and (per_group or not _dense(x)):
+    if not cl and (per_group or not dense(x)):
         x = x.contiguous()
     if layout is None:
         layout = (1, x.shape[0], x.numel() // x.shape[0]) if per_group else (1, 1, x.numel())
@@ -327,11 +363,8 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     if pool is not None:
         # a 2x2 / stride-2 max pooling (floor mode) follows and is the only consumer: computed inside the apply phase
         # ((3, 3): stride 2, padding 1, H and W even - the ResNet stem)
-        # (the per-sample / per-tensor min-max launches take it on channels-last memory when a channel-fastest bias tells
-        # them the channel count)
         rows_cl = any_dense_format and is_cl and bias is not None and bias_period < 0
-        if (tuple(pool) not in ((2, 2), (3, 3)) or not (channels_last or rows_cl) or stats_only or residual is not None or hist is not None
-                or x.shape[3] % 2 or (tuple(pool) == (3, 3) and x.shape[2] % 2)):
+        if not pool_request_ok(x, pool, channels_last or rows_cl, stats_only, residual, hist):
             raise ValueError("pool=(2, 2) / (3, 3) needs a channels-last launch with an even W (3x3: and H) and no residual / histogram")
         n_, c_, h_, w_ = x.shape
         pooled = torch.empty((n_, c_, h_ // 2, w_ // 2), dtype=x.dtype, device=dev, memory_format=torch.channels_last)
@@ -378,7 +411,7 @@ def add_relu_(a, b):
     dense with identical strides (any memory format); returns ``a``.  Bit-identical to the two torch ops."""
     _require_cuda_f32(a, "a")
     _require_cuda_f32(b, "b")
-    if a.shape != b.shape or a.stride() != b.stride() or not _dense(a):
+    if a.shape != b.shape or a.stride() != b.stride() or not dense(a):
         raise ValueError("add_relu_ needs two dense tensors of identical shape and strides")
     with torch.cuda.device(a.device), _Timed("E", a.numel(), 12):
         L.check(L.load().fqb200_add_relu(a.data_ptr(), b.data_ptr(), a.data_ptr(), a.numel(), _stream_handle(a.device)))
