@@ -1086,6 +1086,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 
 }  // namespace fqb
 #include "fq_cl.cuh"
+#include "fq_kld.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1619,6 +1620,11 @@ bool rows_supported(const fqb200_desc* d, bool can_vec) {
 }
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// KLD workspace: [rows] max |x| words, then [rows][num_bins] bin counters (fq_kld.cuh)
+size_t kld_workspace(int64_t rows, int num_bins) {
+  return align_up(static_cast<size_t>(rows) * 4, 256) + static_cast<size_t>(rows) * static_cast<size_t>(num_bins) * 4;
+}
 
 // workspace layout; returns total bytes, fills pointers when base != nullptr.  Partials: one slot per unit.
 size_t carve(char* base, uint64_t slots, uint64_t groups, fqb::FusedArgs* A) {
@@ -2188,6 +2194,76 @@ int fqb200_add_relu(const float* a, const float* b, float* out, int64_t n, void*
   else     fqb::fq_add_relu_kernel<1><<<grid, fqb::kThreads, 0, st>>>(a, b, out, nvec);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_add_relu_kernel: %s", cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+size_t fqb200_kld_workspace_bytes(int64_t rows, int num_bins) {
+  g_err[0] = 0;
+  if (rows <= 0 || rows > (1ll << 31) - 1) return fail(FQB200_ERR_INVALID, "rows must be in 1 .. 2^31 - 1%s"), 0;
+  if (num_bins < 3 || num_bins > 8001 || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s"), 0;
+  return kld_workspace(rows, num_bins);
+}
+
+int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num_bins, int num_quantized_bins, float* out_th,
+                         float* out_div, int32_t* out_idx, void* workspace, size_t workspace_bytes, void* stream) {
+  g_err[0] = 0;
+  if (num_bins < 3 || num_bins > 8001 || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s");
+  if (num_quantized_bins < 3 || num_quantized_bins > num_bins || num_quantized_bins % 2 == 0)
+    return fail(FQB200_ERR_INVALID, "num_quantized_bins must be odd, 3 .. num_bins%s");
+  if (rows <= 0 || row_len <= 0 || rows > (1ll << 31) - 1) return fail(FQB200_ERR_INVALID, "rows / row_len must be positive (rows < 2^31)%s");
+  if (row_len > (1ll << 31) - 1) return fail(FQB200_ERR_UNSUPPORTED, "rows of 2^31 elements and more (int32 bin counts)%s");
+  if (!in || !out_th || !out_div || !out_idx) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  const size_t need = kld_workspace(rows, num_bins);
+  if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15u))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_kld_workspace_bytes() or not 16-byte aligned%s");
+  DeviceInfo* di = nullptr;
+  int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::KldArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.rows = static_cast<unsigned long long>(rows);
+  A.row_len = static_cast<unsigned long long>(row_len);
+  // fill the GPU with (row, chunk) units but keep them long: every unit flushes up to num_bins counters
+  const unsigned long long want = static_cast<unsigned long long>(di->sms) * 4ull;
+  unsigned long long chunks = (want + A.rows - 1) / A.rows;
+  const unsigned long long max_chunks = (A.row_len + 4095ull) / 4096ull;
+  chunks = chunks < max_chunks ? chunks : max_chunks;
+  A.chunk = ((A.row_len + chunks - 1) / chunks + 3ull) / 4ull * 4ull;
+  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
+  A.absmax = static_cast<unsigned*>(workspace);
+  A.hist = reinterpret_cast<unsigned*>(static_cast<char*>(workspace) + align_up(static_cast<size_t>(rows) * 4, 256));
+  A.nb = num_bins;
+  A.nq = num_quantized_bins;
+  int rep = 65536 / (num_bins * 4);
+  A.replicas = rep < 1 ? 1 : (rep > fqb::kKldMaxReplicas ? fqb::kKldMaxReplicas : rep);
+  A.out_th = out_th;
+  A.out_div = out_div;
+  A.out_idx = out_idx;
+  const size_t hist_smem = static_cast<size_t>(A.replicas + 1) * num_bins * 4 + 4;
+  const size_t search_smem = static_cast<size_t>((2 * (num_bins + 1) + 1) & ~1) * 4 + static_cast<size_t>(num_bins / 2 + 1) * 8;
+  const bool vec = row_len % 4 == 0 && aligned16(in);
+  const void* hist_k = vec ? reinterpret_cast<const void*>(fqb::fq_kld_hist_kernel<4>) : reinterpret_cast<const void*>(fqb::fq_kld_hist_kernel<1>);
+  cudaError_t e = cudaFuncSetAttribute(hist_k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hist_smem));
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(reinterpret_cast<const void*>(fqb::fq_kld_search_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             static_cast<int>(search_smem));
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaFuncSetAttribute (KLD kernels): %s", cudaGetErrorString(e));
+  e = cudaMemsetAsync(workspace, 0, need, st);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaMemsetAsync: %s", cudaGetErrorString(e));
+  const unsigned long long units = A.rows * A.chunks;
+  const int grid = static_cast<int>(units < want ? units : want);
+  if (vec) {
+    fqb::fq_kld_absmax_kernel<4><<<grid, fqb::kKldThreads, 0, st>>>(A);
+    fqb::fq_kld_hist_kernel<4><<<grid, fqb::kKldThreads, hist_smem, st>>>(A);
+  } else {
+    fqb::fq_kld_absmax_kernel<1><<<grid, fqb::kKldThreads, 0, st>>>(A);
+    fqb::fq_kld_hist_kernel<1><<<grid, fqb::kKldThreads, hist_smem, st>>>(A);
+  }
+  fqb::fq_kld_search_kernel<<<static_cast<unsigned>(rows), fqb::kKldThreads, search_smem, st>>>(A);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch KLD kernels: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
 

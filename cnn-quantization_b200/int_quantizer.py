@@ -7,8 +7,9 @@ host synchronisations per hooked tensor, every dispatch target below is ONE kern
 memory (contiguous NCHW or channels-last) and never reads anything back to the host.
 
 Scope (SURVEY.md section 8): on-the-fly statistics, offline statistics (``-sm use``: parameters solved once per layer,
-then one apply-only launch), entropy measurement (``-me``, torch and mid-tread grids) and the activation bias
-correction (``-bca``).  Outside the path and raising ``NotImplementedError``: KLD thresholds (``-kld``), ``mix`` clipping.
+then one apply-only launch), KLD thresholds (``-kld``: collected per sample by ops.kld_threshold, applied in use mode as
+one apply-only launch of the compiled leaf), entropy measurement (``-me``, torch and mid-tread grids) and the activation
+bias correction (``-bca``).  Outside the path: ``mix`` clipping.
 """
 import math
 
@@ -150,7 +151,9 @@ class IntQuantizer(object):
                 b = bias.view((1, -1) + (1,) * (tensor.dim() - 2))
                 tensor = tensor.add_(b) if self.inplace else tensor + b
                 bias = None
-            if self.clipping != "no":
+            if self.kld:
+                res = self.gemmlowpKldQuantize(tensor, tag, stat_id=stat_id)
+            elif self.clipping != "no":
                 if self.mtd_quant:
                     res = self.mid_tread_quantize_activation(tensor, id, bias=bias)
                 else:
@@ -185,8 +188,6 @@ class IntQuantizer(object):
     # helpers
     # ------------------------------------------------------------------------------------------
     def _unsupported(self, stat_id):
-        if self.kld:
-            raise NotImplementedError("KLD thresholds are outside the hot-path scope (SURVEY.md section 2, #9)")
         if stat_id is not None and self.sm is None:
             raise RuntimeError("stat_id given but no statistics manager is attached to this quantizer (q.sm)")
 
@@ -499,6 +500,30 @@ class IntQuantizer(object):
             return self._launch(tensor, (1, n, tensor.numel() // n), rows=kw["any_dense_format"], scope=L.SCOPE_TENSOR,
                                 out=self._out(tensor), **kw)
         return self._fused(tensor, (1, 1, tensor.numel()), scope=L.SCOPE_GROUP, out=self._out(tensor), **kw)
+
+    def gemmlowpKldQuantize(self, tensor, tag="", stat_id=None):
+        """Collected KLD threshold as the clipping value, int_quantizer.py:478-486: ('mean' kind) min / max / kld_th / mean
+        -> alpha2DeltaOffset -> the compiled leaf, one apply-only launch.  The float64 arithmetic and the preserve-zero
+        test of __gemmlowpQuantize__ run once per (layer, configuration); the leaf gets them as fp32 scalars, like the
+        reference's pybind call."""
+        if stat_id is None or self.sm is None:
+            raise RuntimeError("KLD quantization (-kld) needs collected statistics: call with stat_id and a statistics "
+                               "manager attached (q.sm, `-sm use`)")
+        key = ("kld", stat_id, self._positive())
+
+        def build():
+            mn, mx, th, mean = (self._stat(stat_id, k, "mean") for k in ("min", "max", "kld_th", "mean"))
+            rng, off = self.alpha2DeltaOffset(th, mx, mn, mean)
+            preserve_zero = bool(self.enforce_true_zero and (off + rng) > 0 and off < 0)
+            return float(rng), float(off), preserve_zero
+
+        rng, off, preserve_zero = self._cached(key, build)
+        if rng <= 0:   # the leaf hands its input back (gemmlowp.cu:31-32)
+            return torch.relu_(tensor) if (self._relu_follows and self.inplace) else (torch.relu(tensor) if self._relu_follows else tensor)
+        if self._bca is not None and tensor.dim() == 4:
+            return self.bias_correction_torch(tensor, ops.float2gemmlowp(tensor, rng, off, self.num_bits, self.int_exp,
+                                                                         preserve_zero, None), bool(self._bca))
+        return ops.float2gemmlowp(tensor, rng, off, self.num_bits, self.int_exp, preserve_zero, None, out=self._out(tensor))
 
     def gemmlowpQuantizeActivationPerChannel(self, tensor, id, tag="", stat_id=None, min_=None, max_=None, bias=None):
         """Per-channel min/max (0 lower bound when positive) with optional bit allocation, int_quantizer.py:409-451."""

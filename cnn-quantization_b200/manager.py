@@ -281,13 +281,16 @@ class QuantizationManagerInference(object):
         if self.stats_mode != "no":
             from .statistics import StatisticManager, StatisticManagerPerChannel
             sf = args.stats_folder if args.stats_folder is not None else args.arch
+            if args.kld_threshold:
+                sf += "_kld_" + args.qtype   # inference_quantization_manager.py:300-301
             base = getattr(args, "stats_base_dir", None)
             if self.stats_mode == "collect":
                 print("Collecting statistics...")
                 if args.per_channel_quant_act:
                     self.stats_manager = StatisticManagerPerChannel(sf, load_stats=False, batch_avg=args.stats_batch_avg, base_dir=base)
                 else:
-                    self.stats_manager = StatisticManager(sf, load_stats=False, batch_avg=args.stats_batch_avg, base_dir=base)
+                    self.stats_manager = StatisticManager(sf, load_stats=False, kld_threshold=args.kld_threshold,
+                                                          batch_avg=args.stats_batch_avg, base_dir=base)
             else:
                 if args.per_channel_quant_act:
                     self._sm_channel = StatisticManagerPerChannel(sf, load_stats=True, base_dir=base)

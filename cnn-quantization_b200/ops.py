@@ -21,7 +21,7 @@ def profile_reset(enable):
 def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
-    'S' statistics only."""
+    'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), which quantizes nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -404,6 +404,41 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
         return (pooled, stats) if want_stats else pooled
     out = _finish_out(kout, uout)
     return (out, stats) if want_stats else out
+
+
+def kld_threshold(x, num_bins=2001, num_quantized_bins=15, return_hist=False):
+    """C ABI fqb200_kld_threshold: the KL-divergence threshold of every sample (dim 0) of ``x``, as the reference's
+    kld_threshold._get_optimal_threshold computes it per sample (numpy 1.x histogram edges, divergence in float64).
+    Returns device tensors ``(th[N], div[N], idx[N])``: the threshold, its divergence and its position in the search
+    (int32); a sample holding NaN / Inf gets NaN, NaN, -1.  With ``return_hist`` the [N, num_bins] int32 bin counts come
+    fourth (a view of the workspace).  Recorded in the launch profile under mode 'K' (two reads of the tensor), apart from
+    the quantization launches."""
+    _require_cuda_f32(x, "tensor")
+    if x.dim() == 0:
+        raise ValueError("kld_threshold needs a tensor with a sample dimension")
+    if not dense(x):
+        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    lib = L.load()
+    dev = x.device
+    rows = x.shape[0]
+    th = torch.empty(rows, dtype=torch.float32, device=dev)
+    div = torch.empty(rows, dtype=torch.float32, device=dev)
+    idx = torch.empty(rows, dtype=torch.int32, device=dev)
+    if rows == 0:
+        return (th, div, idx, torch.zeros((0, num_bins), dtype=torch.int32, device=dev)) if return_hist else (th, div, idx)
+    row_len = x.numel() // rows
+    need = lib.fqb200_kld_workspace_bytes(rows, int(num_bins))
+    if need == 0:
+        L.check(L.ERR_INVALID)
+    # a workspace of its own: the launch zeroes it and fills it with counters (the fused kernels' workspace keeps barriers)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev), _Timed("K", x.numel(), 8, "%dx%d" % (rows, row_len)):
+        L.check(lib.fqb200_kld_threshold(x.data_ptr(), rows, row_len, int(num_bins), int(num_quantized_bins), th.data_ptr(),
+                                         div.data_ptr(), idx.data_ptr(), ws.data_ptr(), ws.numel(), _stream_handle(dev)))
+    if not return_hist:
+        return th, div, idx
+    head = (rows * 4 + 255) // 256 * 256   # the counters follow the rows' max |x| words (fqb200_kld_threshold)
+    return th, div, idx, ws[head:head + rows * num_bins * 4].view(torch.int32).view(rows, num_bins)
 
 
 def add_relu_(a, b):

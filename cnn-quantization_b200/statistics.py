@@ -14,6 +14,8 @@ Collect mode is an offline, one-time pass.  The five statistics the quantizers c
 b, std) come from ONE statistics-only launch of the fused kernel per hooked tensor; the diagnostic columns the
 reference also writes (kurtosis, mean_abs, std_pos) are computed with plain torch ops; the error columns
 (mse_*/cos_*) are NaN exactly as in the reference's own collect runs (it never passes quantized tensors there).
+With ``kld_threshold`` the per-tensor manager adds the ``kld_th`` column: the max over the samples of the KL-divergence
+threshold (ops.kld_threshold, three launches and one read-back per hooked tensor).
 """
 import os
 import pickle
@@ -45,14 +47,15 @@ class StatisticManager(object):
     """Per-tensor statistics (statistic_manager.py:15-178)."""
 
     def __init__(self, folder, load_stats, stats=None, batch_avg=False, kld_threshold=False, collect_err=True, base_dir=None):
-        if kld_threshold:
-            raise NotImplementedError("KLD thresholds are outside the hot-path scope (SURVEY.md section 2, #9)")
         self.name = folder
         self.folder = os.path.join(base_dir or default_base_dir(), "statistics", folder)
         self.stats_names = list(stats) if stats is not None else ["max", "min", "std", "mean", "kurtosis", "mean_abs", "b", "dim"]
         self.batch_avg = batch_avg
         if collect_err:
             self.stats_names += _ERR_COLUMNS
+        self.kld_threshold = kld_threshold
+        if kld_threshold:
+            self.stats_names.append("kld_th")
         self.stats = {}
         self.metadata = {}
         self.save_stats = not load_stats
@@ -85,6 +88,8 @@ class StatisticManager(object):
                 v = torch.mean(flat.abs())
             elif sn == "dim":
                 v = flat.numel()
+            elif sn == "kld_th":
+                v = ops.kld_threshold(t)[0].max()   # the max of the per-sample thresholds (NaN propagates, as np.max)
             else:  # mse_* / cos_*: the reference writes NaN when no quantized tensors are handed in
                 v = float("nan")
             row.append(float(v))

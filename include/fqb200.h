@@ -237,6 +237,23 @@ int fqb200_add_relu(const float* a, const float* b, float* out, int64_t n, void*
 int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* workspace, size_t workspace_bytes,
                  void* stream);
 
+/*
+ * KL-divergence calibration (`-kld` collect, statistic_manager.py:80-82 -> kld_threshold.py:15-80): for each of `rows`
+ * contiguous rows of `row_len` floats (one sample; any dense memory order of it), th = max |x| and a histogram of
+ * `num_bins` bins over (-th, th) with numpy 1.x's edges (float32 of the float64 linspace; th == 0 -> (-0.5, 0.5)), then
+ * the threshold search over the candidates i = num_quantized_bins/2 .. num_bins/2 with the divergence in float64.
+ * Writes per row the threshold out_th = edge[num_bins/2 + 1 + i], its divergence out_div, and out_idx = the candidate's
+ * position in the search (i - num_quantized_bins/2; np.argmin rules: the first NaN, else the first minimum).  A row with a
+ * NaN or Inf gets th = div = NaN and idx = -1.  num_bins odd, 3 .. 8001; num_quantized_bins odd, 3 .. num_bins; row_len
+ * < 2^31.  Three kernel launches on `stream`, no host synchronisation.  The workspace (fqb200_kld_workspace_bytes, 16-byte
+ * aligned) is private to the call: it is zeroed and filled with counters, so it must not be a fqb200_fused workspace.
+ * After the call it holds the histograms: uint32 counts [rows][num_bins] from byte offset (rows * 4 rounded up to 256).
+ */
+int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num_bins, int num_quantized_bins, float* out_th,
+                         float* out_div, int32_t* out_idx, void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace of fqb200_kld_threshold: rows x num_bins counters and rows words (0 and fqb200_last_error() on bad arguments). */
+size_t fqb200_kld_workspace_bytes(int64_t rows, int num_bins);
+
 #ifdef __cplusplus
 }
 #endif
