@@ -20,7 +20,8 @@ STAT_COLUMNS = ("min", "max", "mean", "b", "std", "delta", "offset", "bits", "sc
 SYMBOLS = ("fqb200_abi_version", "fqb200_last_error", "fqb200_resident_ctas", "fqb200_plan_info",
            "fqb200_selftest_division", "fqb200_workspace_bytes", "fqb200_workspace_init", "fqb200_float2gemmlowp",
            "fqb200_quantize1", "fqb200_quantize1_bca", "fqb200_fused", "fqb200_add_relu", "fqb200_maxpool2d_nhwc",
-           "fqb200_kld_threshold", "fqb200_kld_workspace_bytes")
+           "fqb200_kld_threshold", "fqb200_kld_workspace_bytes", "fqb200_sample_sumsq",
+           "fqb200_sample_sumsq_workspace_bytes")
 ABI_VERSION = 3
 
 
@@ -96,6 +97,10 @@ def load():
     lib.fqb200_kld_threshold.argtypes = [vp, i64, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t, vp]
     lib.fqb200_kld_workspace_bytes.restype = ctypes.c_size_t
     lib.fqb200_kld_workspace_bytes.argtypes = [i64, i32]
+    lib.fqb200_sample_sumsq.restype = i32
+    lib.fqb200_sample_sumsq.argtypes = [vp, i64, i64, vp, vp, ctypes.c_size_t, vp]
+    lib.fqb200_sample_sumsq_workspace_bytes.restype = ctypes.c_size_t
+    lib.fqb200_sample_sumsq_workspace_bytes.argtypes = [i64, i64]
     lib.fqb200_plan_info.restype = i32
     lib.fqb200_plan_info.argtypes = [ctypes.POINTER(Desc), ctypes.POINTER(ctypes.c_int64)]
     if lib.fqb200_abi_version() != ABI_VERSION:

@@ -1087,6 +1087,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 }  // namespace fqb
 #include "fq_cl.cuh"
 #include "fq_kld.cuh"
+#include "fq_measure.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1624,6 +1625,13 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 // KLD workspace: [rows] max |x| words, then [rows][num_bins] bin counters (fq_kld.cuh)
 size_t kld_workspace(int64_t rows, int num_bins) {
   return align_up(static_cast<size_t>(rows) * 4, 256) + static_cast<size_t>(rows) * static_cast<size_t>(num_bins) * 4;
+}
+
+// sum-of-squares workspace: one float64 partial per (row, chunk) unit when a row spans several chunks (fq_measure.cuh)
+size_t sumsq_workspace(int64_t rows, int64_t row_len) {
+  const unsigned long long chunk = fqb::sumsq_chunk(static_cast<unsigned long long>(row_len));
+  const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
+  return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * 8 : 0;
 }
 
 // workspace layout; returns total bytes, fills pointers when base != nullptr.  Partials: one slot per unit.
@@ -2264,6 +2272,48 @@ int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num
   fqb::fq_kld_search_kernel<<<static_cast<unsigned>(rows), fqb::kKldThreads, search_smem, st>>>(A);
   e = cudaGetLastError();
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch KLD kernels: %s", cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len) {
+  g_err[0] = 0;
+  if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s"), 0;
+  return sumsq_workspace(rows, row_len);
+}
+
+int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* out, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  g_err[0] = 0;
+  if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s");
+  if (!in || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  const size_t need = sumsq_workspace(rows, row_len);
+  if (need && (!workspace || workspace_bytes < need || !aligned16(workspace)))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_sample_sumsq_workspace_bytes() or not 16-byte aligned%s");
+  if (rows == 0) return FQB200_OK;
+  DeviceInfo* di = nullptr;
+  int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::SumsqArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.rows = static_cast<unsigned long long>(rows);
+  A.row_len = static_cast<unsigned long long>(row_len);
+  A.chunk = fqb::sumsq_chunk(A.row_len);
+  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  const unsigned long long units = A.rows * A.chunks;
+  const unsigned long long cap = static_cast<unsigned long long>(di->sms) * (2048ull / fqb::kSumsqThreads);
+  const int grid = static_cast<int>(units < cap ? units : cap);
+  if (row_len % 4 == 0 && aligned16(in)) fqb::fq_sumsq_partial_kernel<4><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
+  else                                   fqb::fq_sumsq_partial_kernel<1><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
+  if (A.chunks > 1) {
+    const unsigned long long blocks = (A.rows + fqb::kSumsqThreads - 1) / fqb::kSumsqThreads;
+    fqb::fq_sumsq_finish_kernel<<<static_cast<unsigned>(blocks), fqb::kSumsqThreads, 0, st>>>(A);
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch sum-of-squares kernels: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
 

@@ -136,6 +136,8 @@ def set_node_names(model):
 # the manager
 # ---------------------------------------------------------------------------------------------------
 _STAMPED = (nn.Linear, nn.Conv2d, nn.BatchNorm2d, nn.MaxPool2d, nn.AvgPool2d)
+# the call sites `-ms` measures (inference_quantization_manager.py:209-210, 247-248, 280-281): not the poolings
+_MEASURED = {nn.Conv2d: "conv%d_activation", nn.Linear: "linear%d_activation", nn.BatchNorm2d: "bn%d_activation"}
 
 
 def _identity_forward(x):
@@ -275,6 +277,18 @@ class QuantizationManagerInference(object):
         # channels-last max pooling in front of the `activation_pooling` call site runs on this package's kernel
         self.fast_maxpool = self._native
         self.inplace_activations = self._native
+        # `-ms` (inference_quantization_manager.py:320-323): the per-sample squared norm of the tensor every conv / linear /
+        # non-absorbed BN call site hands on.  Three launches never write that tensor - the block epilogue writes
+        # max(q + identity, 0), a deferred shortcut is quantized only inside the consuming launch, a pooling launch writes
+        # the pooled quarter - so they are switched off; each is bit-identical to its unfused form.
+        self.measure_stats = None
+        if args.measure_stats:
+            import torch.distributed as dist
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                raise NotImplementedError("-ms with several ranks: per-rank shards would put the rows out of sample order")
+            from .statistics import MeasureStatistics
+            self.measure_stats = MeasureStatistics(args.arch, getattr(args, "stats_base_dir", None))
+            self.fuse_residual_into_quant = self.defer_shortcut = self.fuse_pool_into_quant = False
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None
         self._sm_tensor = self._sm_channel = None
@@ -413,6 +427,8 @@ class QuantizationManagerInference(object):
         self.detach()
         if self.stats_manager is not None:
             self.stats_manager.__exit__()  # collect mode: write the CSV / pickle files
+        if self.measure_stats is not None:
+            self.measure_stats.__exit__()  # -ms: write distance.csv
 
     # -- call sites: forward hooks reproducing the *WithId.forward bodies (:58-74, :84-101, :162-217, :227-250, :262-283)
     def attach(self, model):
@@ -483,6 +499,8 @@ class QuantizationManagerInference(object):
                 self._debiased.append(m)
             hook = {nn.Conv2d: self._conv_hook, nn.Linear: self._linear_hook, nn.MaxPool2d: self._maxpool_hook,
                     nn.AvgPool2d: self._avgpool_hook, nn.BatchNorm2d: self._bn_hook}[cls]
+            if self.measure_stats is not None and cls in _MEASURED:
+                hook = self._measuring(hook, _MEASURED[cls])
             self._hooks.append(m.register_forward_hook(hook))
         return model
 
@@ -504,6 +522,18 @@ class QuantizationManagerInference(object):
             del m._fq_bias_param
             m.bias = param
         self._debiased = []
+
+    def _measuring(self, hook, id_format):
+        """``hook`` followed by the `-ms` measurement of what the call site hands on: the hook's result, or ``out`` where
+        the hook leaves it (collect mode, quantization disabled).  Measured whether or not quantization is enabled, as the
+        reference's *WithId modules do; an absorbed BN (the identity) is not a measured site."""
+        def measured(m, inputs, out):
+            res = hook(m, inputs, out)
+            if not (isinstance(m, nn.BatchNorm2d) and self.bn_folding and hasattr(m, "absorbed")):
+                self.measure_stats.save_measure(out if res is None else res, id_format % m._fq_id)
+            return res
+
+        return measured
 
     def _stat_id(self, activation_id):
         return activation_id if self.stats_mode == "use" else None

@@ -21,7 +21,8 @@ def profile_reset(enable):
 def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
-    'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), which quantizes nothing."""
+    'S' statistics only; 'K' the KLD calibration (ops.kld_threshold) and 'M' the activation norm measurement
+    (ops.sample_sumsq), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -439,6 +440,31 @@ def kld_threshold(x, num_bins=2001, num_quantized_bins=15, return_hist=False):
         return th, div, idx
     head = (rows * 4 + 255) // 256 * 256   # the counters follow the rows' max |x| words (fqb200_kld_threshold)
     return th, div, idx, ws[head:head + rows * num_bins * 4].view(torch.int32).view(rows, num_bins)
+
+
+def sample_sumsq(x):
+    """C ABI fqb200_sample_sumsq: ``x.double().pow(2).sum()`` of every sample (dim 0) of ``x`` as a float64 [N] device
+    tensor - the activation norm `-ms` records (distance_stats.py:27-28).  Deterministic (fixed chunks, fixed summation
+    order), no host synchronisation.  Recorded in the launch profile under mode 'M' (one read of the tensor), apart from
+    the quantization launches."""
+    _require_cuda_f32(x, "tensor")
+    if x.dim() == 0:
+        raise ValueError("sample_sumsq needs a tensor with a sample dimension")
+    if not dense(x):
+        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    dev = x.device
+    rows = x.shape[0]
+    if rows == 0 or x.numel() == 0:
+        return torch.zeros(rows, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
+    lib = L.load()
+    row_len = x.numel() // rows
+    out = torch.empty(rows, dtype=torch.float64, device=dev)
+    need = lib.fqb200_sample_sumsq_workspace_bytes(rows, row_len)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev) if need else None
+    with torch.cuda.device(dev), _Timed("M", x.numel(), 4, "%dx%d" % (rows, row_len)):
+        L.check(lib.fqb200_sample_sumsq(x.data_ptr(), rows, row_len, out.data_ptr(), ws.data_ptr() if ws is not None else None,
+                                        need, _stream_handle(dev)))
+    return out
 
 
 def add_relu_(a, b):

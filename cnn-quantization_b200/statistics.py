@@ -16,6 +16,12 @@ reference also writes (kurtosis, mean_abs, std_pos) are computed with plain torc
 (mse_*/cos_*) are NaN exactly as in the reference's own collect runs (it never passes quantized tensors there).
 With ``kld_threshold`` the per-tensor manager adds the ``kld_th`` column: the max over the samples of the KL-divergence
 threshold (ops.kld_threshold, three launches and one read-back per hooked tensor).
+
+``MeasureStatistics`` is the activation norm measurement (`-ms`, distance_stats.py:15-54):
+
+    <base>/distance/<folder>/distance.csv                       columns = ids in first-call order, one row per sample
+
+Each hooked tensor costs one ops.sample_sumsq launch; the results stay on the device until ``__exit__``.
 """
 import os
 import pickle
@@ -27,7 +33,7 @@ import torch
 
 from . import ops
 
-__all__ = ["StatisticManager", "StatisticManagerPerChannel", "default_base_dir"]
+__all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "default_base_dir"]
 
 
 def default_base_dir():
@@ -224,3 +230,44 @@ class StatisticManagerPerChannel(object):
 
     def __enter__(self):
         return self
+
+
+class MeasureStatistics(object):
+    """Per-sample squared L2 norm of every measured tensor (distance_stats.py:15-54): ``save_measure(t, id)`` records
+    sum(t[i]**2) for every sample i; ``__exit__`` writes them, rounded to float32 (the reference sums in float32), as one
+    column per id in first-call order and one row per sample in call order."""
+
+    def __init__(self, folder, base_dir=None):
+        self.folder = os.path.join(base_dir or default_base_dir(), "distance", folder)
+        self.stats = {}   # id -> float64 [N] tensors, one per call
+        self.stats_names = ["dist"]
+
+    def save_measure(self, tensor, id):
+        t = tensor.detach()
+        if t.is_cuda:
+            d = ops.sample_sumsq(t)   # enqueued now: later in-place writes to the tensor come after it in stream order
+        else:
+            d = t.reshape(t.shape[0], -1).double().pow(2).sum(-1)
+        self.stats.setdefault(id, []).append(d)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *args):
+        if not self.stats:
+            return
+        import pandas as pd
+        cols = list(self.stats)
+        per_id = [torch.cat(v) for v in self.stats.values()]
+        rows = per_id[0].numel()
+        if any(c.numel() != rows for c in per_id):
+            raise ValueError("-ms: the measured ids saw different numbers of samples: %s"
+                             % {k: c.numel() for k, c in zip(cols, per_id)})
+        dev = per_id[0].device
+        # one device-to-host copy for all ids; float32 like the reference's values, written as its float64 column dtype
+        table = torch.stack([c.to(dev) for c in per_id]).float().cpu().numpy().astype(np.float64)
+        if os.path.exists(self.folder):
+            shutil.rmtree(self.folder)
+        os.makedirs(self.folder)
+        pd.DataFrame(data=table.T, columns=cols).to_csv(os.path.join(self.folder, "distance.csv"), index=False)
+        self.stats = {}

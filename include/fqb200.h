@@ -254,6 +254,19 @@ int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num
 /* Workspace of fqb200_kld_threshold: rows x num_bins counters and rows words (0 and fqb200_last_error() on bad arguments). */
 size_t fqb200_kld_workspace_bytes(int64_t rows, int num_bins);
 
+/*
+ * Activation norm measurement (`-ms`, distance_stats.py:22-33): out[r] = the float64 sum of x * x over row r, for `rows`
+ * contiguous rows of `row_len` floats (one sample; any dense memory order of it).  Work units are (row, chunk) with a
+ * chunk length that depends on row_len only; each unit's partial goes to the workspace and a row's partials are added in
+ * chunk order, so the result has the same bits on every run.  NaN and Inf propagate; rows == 0 launches nothing.  One
+ * read of the tensor plus, when a row spans several chunks, a small second launch, on `stream`; no host synchronisation.
+ * The workspace (fqb200_sample_sumsq_workspace_bytes, 16-byte aligned; may be null when that is 0) is private to the call.
+ */
+int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* out, void* workspace, size_t workspace_bytes,
+                        void* stream);
+/* Workspace of fqb200_sample_sumsq in bytes (0 and fqb200_last_error() on bad arguments: rows < 0, row_len <= 0). */
+size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len);
+
 #ifdef __cplusplus
 }
 #endif
