@@ -244,28 +244,35 @@ __device__ __noinline__ void solve_bit_alloc(const FusedArgs& A, LeaderSmem& sm)
   cta_sync();
 }
 
+// Internal range rule of the clipping-error candidates (fq_cliperr.cuh), not a public FQB200_RANGE_* value: the `lowp`
+// alpha of get_alpha(clip_type='mix'), (max - min) / 2 (int_quantizer.py:320), through alpha2DeltaOffset like the others.
+constexpr int kRangeLowp = -1;
+
 // (delta, offset) of one group/tensor from its statistics: int_quantizer.py:284-300 (alpha2DeltaOffset),
 // :227-275 (alpha), :348-352 / :354-357 (fp32 per-channel vs float64 per-tensor arithmetic), :361-379, :409-424.
-__device__ __forceinline__ void solve_range(const FusedArgs& A, float mn, float mx, float mean, float b, float sd,
-                                            float bits, float& delta, float& offset) {
-  if (A.range_mode == FQB200_RANGE_MINMAX) {
-    offset = A.positive ? 0.f : mn;
+__device__ __forceinline__ void solve_range(int range_mode, bool positive, int num_bits, float clip_k, bool solve_f64,
+                                            float mn, float mx, float mean, float b, float sd, float bits, float& delta,
+                                            float& offset) {
+  if (range_mode == FQB200_RANGE_MINMAX) {
+    offset = positive ? 0.f : mn;
     delta = __fsub_rn(mx, offset);
     return;
   }
   float alpha;
   const int bi = static_cast<int>(bits);
-  if (A.range_mode == FQB200_RANGE_LAPLACE) {
-    alpha = __fmul_rn(b, A.positive ? kLaplacePos[bi] : kLaplace[bi]);
-  } else if (A.range_mode == FQB200_RANGE_GAUS) {
-    alpha = __fmul_rn(sd, A.positive ? kGausPos[A.num_bits] : kGaus[A.num_bits]);
+  if (range_mode == FQB200_RANGE_LAPLACE) {
+    alpha = __fmul_rn(b, positive ? kLaplacePos[bi] : kLaplace[bi]);
+  } else if (range_mode == FQB200_RANGE_GAUS) {
+    alpha = __fmul_rn(sd, positive ? kGausPos[num_bits] : kGaus[num_bits]);
+  } else if (range_mode == kRangeLowp) {
+    alpha = __fmul_rn(__fsub_rn(mx, mn), 0.5f);   // = RN((mx - mn) / 2)
   } else {
-    alpha = __fmul_rn(A.clip_k, sd);
+    alpha = __fmul_rn(clip_k, sd);
   }
-  if (A.solve_f64) {
+  if (solve_f64) {
     const double al = alpha, me = mean;
     double dl, of;
-    if (A.positive) {
+    if (positive) {
       dl = fmax(me, 0.0) + al;
       of = 0.0;
     } else {
@@ -275,7 +282,7 @@ __device__ __forceinline__ void solve_range(const FusedArgs& A, float mn, float 
     delta = static_cast<float>(dl);
     offset = static_cast<float>(of);
   } else {
-    if (A.positive) {
+    if (positive) {
       delta = __fadd_rn(fmaxf(mean, 0.f), alpha);
       offset = 0.f;
     } else {
@@ -285,6 +292,11 @@ __device__ __forceinline__ void solve_range(const FusedArgs& A, float mn, float 
       delta = __fsub_rn(__fadd_rn(offset, rng), offset);
     }
   }
+}
+__device__ __forceinline__ void solve_range(const FusedArgs& A, float mn, float mx, float mean, float b, float sd,
+                                            float bits, float& delta, float& offset) {
+  solve_range(A.range_mode, A.positive != 0, A.num_bits, A.clip_k, A.solve_f64 != 0, mn, mx, mean, b, sd, bits, delta,
+              offset);
 }
 
 // leaf parameters from (delta, offset, bits)
@@ -1088,6 +1100,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_cl.cuh"
 #include "fq_kld.cuh"
 #include "fq_measure.cuh"
+#include "fq_cliperr.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1632,6 +1645,16 @@ size_t sumsq_workspace(int64_t rows, int64_t row_len) {
   const unsigned long long chunk = fqb::sumsq_chunk(static_cast<unsigned long long>(row_len));
   const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
   return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * 8 : 0;
+}
+
+// clipping-error workspace: kCeSums float64 partials per (group, unit) (fq_cliperr.cuh)
+unsigned long long cliperr_units_per_group(int64_t outer, int64_t inner, int channels_last) {
+  const unsigned long long n = static_cast<unsigned long long>(outer) * static_cast<unsigned long long>(inner);
+  const unsigned long long per = channels_last ? fqb::kCeClRows : fqb::kCeChunk;
+  return (n + per - 1) / per;
+}
+size_t cliperr_workspace(int64_t outer, int64_t groups, int64_t inner, int channels_last) {
+  return static_cast<size_t>(groups) * static_cast<size_t>(cliperr_units_per_group(outer, inner, channels_last)) * fqb::kCeSums * 8;
 }
 
 // workspace layout; returns total bytes, fills pointers when base != nullptr.  Partials: one slot per unit.
@@ -2314,6 +2337,67 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch sum-of-squares kernels: %s", cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+// the layouts fqb200_clip_error takes (argument errors as a message, nullptr when they are fine)
+static const char* cliperr_bad_args(int64_t outer, int64_t groups, int64_t inner, int channels_last) {
+  if (outer <= 0 || groups <= 0 || inner <= 0) return "outer, groups and inner must be > 0%s";
+  if (channels_last && !flat_eligible(groups)) return "channels_last needs C %% 4 == 0 and 4 <= C <= 2048%s";
+  if (!channels_last && outer > 1 && static_cast<unsigned long long>(outer) * static_cast<unsigned long long>(inner) >= (1ull << 32))
+    return "a group of an NCHW layout must hold fewer than 2^32 elements%s";
+  return nullptr;
+}
+
+size_t fqb200_clip_error_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last) {
+  g_err[0] = 0;
+  const char* bad = cliperr_bad_args(outer, groups, inner, channels_last);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  return cliperr_workspace(outer, groups, inner, channels_last);
+}
+
+int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last, const float* stats,
+                      int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, double* out, float* out_params,
+                      void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  const char* bad = cliperr_bad_args(outer, groups, inner, channels_last);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!in || !stats || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
+  if (bit_alloc && num_bits > 4) return fail(FQB200_ERR_INVALID, "bit_alloc applies to num_bits <= 4 only%s");
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  const size_t need = cliperr_workspace(outer, groups, inner, channels_last);
+  if (!workspace || workspace_bytes < need || !aligned16(workspace))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_clip_error_workspace_bytes() or not 16-byte aligned%s");
+  DeviceInfo* di = nullptr;
+  int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::ClipErrArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.stats = stats;
+  A.outer = static_cast<unsigned long long>(outer);
+  A.groups = static_cast<unsigned long long>(groups);
+  A.inner = static_cast<unsigned long long>(inner);
+  A.channels_last = channels_last ? 1 : 0;
+  A.num_bits = num_bits;
+  A.positive = positive ? 1 : 0;
+  A.bit_alloc = bit_alloc ? 1 : 0;
+  A.solve_f64 = solve_f64 ? 1 : 0;
+  A.units_per_group = cliperr_units_per_group(outer, inner, channels_last);
+  A.units = A.units_per_group * (channels_last ? (A.groups + fqb::kCeSlab - 1) / fqb::kCeSlab : A.groups);
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  A.params = out_params;
+  const unsigned long long cap = max_ctas ? static_cast<unsigned long long>(max_ctas)
+                                          : static_cast<unsigned long long>(di->sms) * (2048ull / fqb::kCeThreads);
+  const int grid = static_cast<int>(A.units < cap ? A.units : cap);
+  if (!channels_last && inner % 4 == 0 && aligned16(in)) fqb::fq_cliperr_partial_kernel<4><<<grid, fqb::kCeThreads, 0, st>>>(A);
+  else                                                   fqb::fq_cliperr_partial_kernel<1><<<grid, fqb::kCeThreads, 0, st>>>(A);
+  fqb::fq_cliperr_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCeThreads, 0, st>>>(A);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch clipping-error kernels: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
 

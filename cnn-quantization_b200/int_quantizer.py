@@ -9,7 +9,8 @@ memory (contiguous NCHW or channels-last) and never reads anything back to the h
 Scope (SURVEY.md section 8): on-the-fly statistics, offline statistics (``-sm use``: parameters solved once per layer,
 then one apply-only launch), KLD thresholds (``-kld``: collected per sample by ops.kld_threshold, applied in use mode as
 one apply-only launch of the compiled leaf), entropy measurement (``-me``, torch and mid-tread grids) and the activation
-bias correction (``-bca``).  Outside the path: ``mix`` clipping.
+bias correction (``-bca``) and ``mix`` clipping (``-sm use`` only: the per-layer or per-channel choice between no clipping,
+Gauss and Laplace by the mse_* statistics collected with ``collect_err``, then one apply-only launch).
 """
 import math
 
@@ -387,23 +388,10 @@ class IntQuantizer(object):
             dev = tensor.device
             mn, mx, mean = (self._stat(stat_id, k, "mean") for k in ("min", "max", "mean"))
             per_channel = pc_shape and np.size(mn) > 1 and np.size(mx) > 1
-            table_l = self.alpha_laplace_positive if positive else self.alpha_laplace
-            table_g = self.alpha_gaus_positive if positive else self.alpha_gaus
-            bits = None
-            if clip_type == "laplace":
-                b = self._stat(stat_id, "b", "mean")
-                if self.bit_alloc_act and per_channel and self.num_bits <= 4:
-                    bits = self._stat_bits(stat_id, dev, self.bit_alloc_target_act)
-                    factor = torch.tensor(np.array([table_l[int(v)] for v in bits.tolist()]), dtype=torch.float32, device=dev)
-                else:
-                    factor = table_l[self.num_bits]
-                alpha = _to_dev(np.asarray(b, dtype=np.float32) if per_channel else b, dev) * factor
-            elif clip_type == "gaus":
-                alpha = self._stat(stat_id, "std", "mean") * table_g[self.num_bits]
-            elif "std" in clip_type:
-                alpha = float(clip_type.replace("std", "")) * self._stat(stat_id, "std", "mean")
+            if clip_type == "mix":
+                alpha, bits = self._mix_alpha_from_stats(stat_id, per_channel, dev)
             else:
-                raise NotImplementedError("clipping %r is not supported with offline statistics" % clip_type)
+                alpha, bits = self._alpha_from_stats(stat_id, clip_type, per_channel, dev)
             if per_channel:
                 rng, off = self.alpha2DeltaOffset(alpha if isinstance(alpha, torch.Tensor) else np.asarray(alpha, dtype=np.float32),
                                                   np.asarray(mx, dtype=np.float32), np.asarray(mn, dtype=np.float32),
@@ -422,6 +410,51 @@ class IntQuantizer(object):
                     None, False)
 
         return self._cached(key, build)
+
+    def _alpha_from_stats(self, stat_id, clip_type, per_channel, dev):
+        """(alpha, allocated bits or None) of get_alpha with collected statistics (int_quantizer.py:227-275, :320), in the
+        reference's types: the Laplace alpha is an fp32 device tensor, the others numpy / pandas values."""
+        positive = self._positive()
+        bits = None
+        if clip_type == "laplace":
+            table_l = self.alpha_laplace_positive if positive else self.alpha_laplace
+            b = self._stat(stat_id, "b", "mean")
+            if self.bit_alloc_act and per_channel and self.num_bits <= 4:
+                bits = self._stat_bits(stat_id, dev, self.bit_alloc_target_act)
+                factor = torch.tensor(np.array([table_l[int(v)] for v in bits.tolist()]), dtype=torch.float32, device=dev)
+            else:
+                factor = table_l[self.num_bits]
+            return _to_dev(np.asarray(b, dtype=np.float32) if per_channel else b, dev) * factor, bits
+        if clip_type == "gaus":
+            return self._stat(stat_id, "std", "mean") * (self.alpha_gaus_positive if positive else self.alpha_gaus)[self.num_bits], bits
+        if clip_type == "lowp":   # `mix`'s no-clipping candidate
+            return (self._stat(stat_id, "max", "mean") - self._stat(stat_id, "min", "mean")) / 2, bits
+        if "std" in clip_type:
+            return float(clip_type.replace("std", "")) * self._stat(stat_id, "std", "mean"), bits
+        raise NotImplementedError("clipping %r is not supported with offline statistics" % clip_type)
+
+    def _mix_alpha_from_stats(self, stat_id, per_channel, dev):
+        """`-c mix` (int_quantizer.py:310-323), elementwise per tensor or per channel, with the reference's order: Gauss
+        where mse_gaus < mse_laplace, else Laplace; then lowp wherever mse_lowp < mse_gaus (even when Laplace beats both).
+        Ties keep the earlier choice; NaN errors (statistics collected without them) select Laplace."""
+        try:
+            mse = {k: np.asarray(self._stat(stat_id, "mse_" + k, "mean"), dtype=np.float64) for k in ("lowp", "gaus", "laplace")}
+        except KeyError:
+            raise KeyError("-c mix needs the mse_* statistics of layer %r: collect them with collect_err=True" % (stat_id,))
+
+        def host(a):
+            return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+
+        a_laplace, bits = self._alpha_from_stats(stat_id, "laplace", per_channel, dev)
+        a_gaus = self._alpha_from_stats(stat_id, "gaus", per_channel, dev)[0]
+        a_lowp = self._alpha_from_stats(stat_id, "lowp", per_channel, dev)[0]
+        alpha = np.where(mse["gaus"] < mse["laplace"], host(a_gaus), host(a_laplace))
+        alpha = np.where(mse["lowp"] < mse["gaus"], host(a_lowp), alpha)
+        if per_channel:
+            alpha = alpha.astype(np.float32)
+        if bits is None and self.bit_alloc_act and per_channel and self.num_bits <= 4:
+            bits = self._stat_bits(stat_id, dev, self.bit_alloc_target_act)
+        return alpha, bits
 
     # ------------------------------------------------------------------------------------------
     # dispatch targets
@@ -801,7 +834,12 @@ class IntQuantizer(object):
         return p * stats(tensor, ["std"])["std"]
 
     def get_alpha(self, tensor, tag="", stat_id=None, clip_type="laplace", per_channel=False):
-        """int_quantizer.py:302-325."""
+        """int_quantizer.py:302-325.  ``mix`` needs collected statistics (``stat_id`` and ``sm``), as in the reference."""
+        if clip_type == "mix":
+            if stat_id is None or self.sm is None:
+                raise NotImplementedError("clipping 'mix' chooses by collected errors: it needs stat_id and a statistics "
+                                          "manager (-sm use with statistics collected with collect_err=True)")
+            return self._mix_alpha_from_stats(stat_id, per_channel, tensor.device)[0]
         if clip_type == "laplace":
             return self.get_alpha_laplace(tensor, stat_id, per_channel=per_channel)
         if clip_type == "gaus":

@@ -19,6 +19,7 @@ from itertools import count
 import torch
 import torch.nn as nn
 
+from . import _lib as L
 from .dummy_quantizer import DummyQuantizer
 from .int_quantizer import int_quantizer as _default_factory
 
@@ -30,13 +31,15 @@ FUSED_RELU_ARCHS = ("alexnet", "vgg16", "vgg16_bn", "inception_v3")
 
 def make_args(**over):
     """An ``args`` namespace with the reference CLI's defaults (inference/inference_sim.py:52-112) for the fields the
-    manager and the quantizers read."""
+    manager and the quantizers read.  Extensions without a reference flag: ``stats_base_dir`` and ``collect_err`` (fill the
+    mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument)."""
     d = dict(arch="resnet18", qtype=None, qweight="int8", q_off=False, clipping="no", stats_mode="no", stats_kind="mean",
              stats_folder=None, stats_batch_avg=False, kld_threshold=False, measure_stats=False,
              per_channel_quant_weights=False, per_channel_quant_act=False, bit_alloc_act=False, bit_alloc_weight=False,
              bit_alloc_rmode="round", bit_alloc_prior="gaus", bit_alloc_target_act=None, bit_alloc_target_weight=None,
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
-             mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None)
+             mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
+             collect_err=False)
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -289,6 +292,12 @@ class QuantizationManagerInference(object):
             from .statistics import MeasureStatistics
             self.measure_stats = MeasureStatistics(args.arch, getattr(args, "stats_base_dir", None))
             self.fuse_residual_into_quant = self.defer_shortcut = self.fuse_pool_into_quant = False
+        # `collect_err`: the collect hooks hand each tensor's use-mode quantizer settings to save_tensor_stats, which fills
+        # the mse_* / cos_* columns `-c mix` chooses by
+        self.collect_err = bool(getattr(args, "collect_err", False))
+        if self.collect_err and (self.stats_mode != "collect" or args.qtype is None):
+            raise ValueError("collect_err fills error columns of -sm collect for the bit widths of -qtype: it needs "
+                             "stats_mode='collect' and a qtype (got stats_mode=%r, qtype=%r)" % (self.stats_mode, args.qtype))
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None
         self._sm_tensor = self._sm_channel = None
@@ -301,7 +310,8 @@ class QuantizationManagerInference(object):
             if self.stats_mode == "collect":
                 print("Collecting statistics...")
                 if args.per_channel_quant_act:
-                    self.stats_manager = StatisticManagerPerChannel(sf, load_stats=False, batch_avg=args.stats_batch_avg, base_dir=base)
+                    self.stats_manager = StatisticManagerPerChannel(sf, load_stats=False, batch_avg=args.stats_batch_avg,
+                                                                    collect_err=self.collect_err, base_dir=base)
                 else:
                     self.stats_manager = StatisticManager(sf, load_stats=False, kld_threshold=args.kld_threshold,
                                                           batch_avg=args.stats_batch_avg, base_dir=base)
@@ -535,6 +545,21 @@ class QuantizationManagerInference(object):
 
         return measured
 
+    def _clip_err(self, out, tag, stat_id, half_range):
+        """``save_tensor_stats`` kwargs of a collect call site: with collect_err, the settings of the quantizer
+        quantize_instant picks for the same call in `-sm use` (``tag``, the 8-bit ``ignored`` list, ``half_range``) on
+        this tensor ``out``: per channel when it would quantize it per channel, with bit allocation only then."""
+        if not self.collect_err:
+            return {}
+        from .statistics import ClipErrConfig
+        q = self.get_quantizer("ignored" if stat_id in self.ignore_ids else tag)
+        per_channel = bool(q.pcq_a and out.dim() == 4 and (out.shape[2] > 1 or out.shape[3] > 1) and out.shape[1] > 1)
+        return {"clip_err": ClipErrConfig(num_bits=min(q.num_bits, 8), positive=bool(q.force_positive or half_range),
+                                          per_channel=per_channel,
+                                          bit_alloc=bool(per_channel and q.bit_alloc_act and q.num_bits <= 4),
+                                          bit_alloc_prior=L.PRIOR_STD if q.bit_alloc_prior == "gaus" else L.PRIOR_B,
+                                          bit_alloc_round=bool(q.bit_alloc_round), bit_alloc_target=q.bit_alloc_target_act)}
+
     def _stat_id(self, activation_id):
         return activation_id if self.stats_mode == "use" else None
 
@@ -544,11 +569,12 @@ class QuantizationManagerInference(object):
             return None if bias is None else out + bias.view(1, -1, 1, 1)
         activation_id = "conv%d_activation" % m._fq_id
         tag = "activation_classifier" if out.shape[1] == 1000 else "activation"
+        half_range = hasattr(m, "before_relu")
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, getattr(m, "internal_name", activation_id), activation_id)
+            self.stats_manager.save_tensor_stats(out, getattr(m, "internal_name", activation_id), activation_id,
+                                                 **self._clip_err(out, tag, activation_id, half_range))
             return None
         extra = {} if bias is None else {"bias": bias}
-        half_range = hasattr(m, "before_relu")
         if self.stats_mode == "use" and self.bcorr_act:
             # `-bca` (:180-196): the correction runs inside the quantizer's given-parameter launch
             return self.quantize_instant(out, activation_id, tag, stat_id=activation_id, half_range=half_range,
@@ -592,10 +618,11 @@ class QuantizationManagerInference(object):
         classifier = m.weight.shape[0] == 1000
         activation_id = "linear%d_activation" % m._fq_id
         tag = "activation_classifier" if classifier else "activation_linear"
-        if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, tag, activation_id, force_global_min_max=("classifier" in tag))
-            return None
         half_range = hasattr(m, "before_relu") if not classifier else False
+        if self.stats_mode == "collect":
+            self.stats_manager.save_tensor_stats(out, tag, activation_id, force_global_min_max=("classifier" in tag),
+                                                 **self._clip_err(out, tag, activation_id, half_range))
+            return None
         return self.quantize_instant(out, activation_id, tag, stat_id=self._stat_id(activation_id), half_range=half_range,
                                      verbose=self.verbose)
 
@@ -604,7 +631,8 @@ class QuantizationManagerInference(object):
             return None
         out_id = "maxpool%d_out" % m._fq_id
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, "activation_pooling", out_id)
+            self.stats_manager.save_tensor_stats(out, "activation_pooling", out_id,
+                                                 **self._clip_err(out, "activation_pooling", out_id, False))
             return None
         return self.quantize_instant(out, out_id, "activation_pooling", stat_id=self._stat_id(out_id), verbose=self.verbose)
 
@@ -614,7 +642,7 @@ class QuantizationManagerInference(object):
         out_id = "avgpool%d_out" % m._fq_id
         tag_act = "activation_classifier" if out.shape[1] == 1000 else "activation_pooling"
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, tag_act, out_id)
+            self.stats_manager.save_tensor_stats(out, tag_act, out_id, **self._clip_err(out, "", out_id, False))
             return None
         # the reference passes the tag in the id slot here (:96,:99): the tensor goes through the DEFAULT quantizer
         return self.quantize_instant(out, tag_act, stat_id=self._stat_id(out_id), verbose=self.verbose)
@@ -626,7 +654,8 @@ class QuantizationManagerInference(object):
             return None
         activation_id = "bn%d_activation" % m._fq_id
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, "activation", activation_id)
+            self.stats_manager.save_tensor_stats(out, "activation", activation_id,
+                                                 **self._clip_err(out, "", activation_id, hasattr(m, "before_relu")))
             return None
         # same argument-order slip as the reference (:275,:278): id="activation", tag="" -> default quantizer
         return self.quantize_instant(out, "activation", stat_id=self._stat_id(activation_id),

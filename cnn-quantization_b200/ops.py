@@ -21,8 +21,8 @@ def profile_reset(enable):
 def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
-    'S' statistics only; 'K' the KLD calibration (ops.kld_threshold) and 'M' the activation norm measurement
-    (ops.sample_sumsq), which quantize nothing."""
+    'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
+    (ops.sample_sumsq) and 'E' the clipping-error measurement (ops.clip_error), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -465,6 +465,54 @@ def sample_sumsq(x):
         L.check(lib.fqb200_sample_sumsq(x.data_ptr(), rows, row_len, out.data_ptr(), ws.data_ptr() if ws is not None else None,
                                         need, _stream_handle(dev)))
     return out
+
+
+CLIP_ERROR_CANDIDATES = ("lowp", "gaus", "laplace")
+
+
+def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=False, solve_f64=None, want_params=False,
+               max_ctas=0):
+    """C ABI fqb200_clip_error: per group of ``layout`` = (outer, groups, inner), the float64 sums behind the mse_* / cos_*
+    statistics of the three candidates ``CLIP_ERROR_CANDIDATES`` of `-c mix`, as a [groups, 10] device tensor: column 0
+    sum x^2, 1 + k sum (x - q_k)^2, 4 + k sum x * q_k, 7 + k sum q_k^2.  ``table`` is the [groups, 12] table of a
+    ``fused(..., stats_only=True)`` launch on the same tensor and layout (with ``bit_alloc``, one configured with the same
+    bit allocation: its column 7 holds the widths); the candidates' parameters are solved from it on the device, in float64
+    when ``solve_f64`` (default: a single group) else fp32.  ``channels_last``: per-channel groups of an ``cl_eligible``
+    tensor, read in place; other per-channel tensors are read as NCHW (copied when not contiguous).  Deterministic, no
+    host synchronisation; with ``want_params`` also returns the [groups, 3, 6] candidate parameters (delta, offset, bits,
+    scale, zero point, qmax).  Recorded in the launch profile under mode 'E' (one read of the tensor)."""
+    _require_cuda_f32(x, "tensor")
+    outer, groups, inner = (int(v) for v in layout)
+    if outer * groups * inner != x.numel():
+        raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
+    if channels_last:
+        if not cl_eligible(x, layout):
+            raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
+    elif not (outer == 1 and groups == 1 and dense(x)):
+        x = x.contiguous()   # one group: any dense memory order; per channel: NCHW order
+    if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
+            or tuple(table.shape) != (groups, L.STATS_STRIDE)):
+        raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
+    table = table.contiguous()
+    lib = L.load()
+    dev = x.device
+    if solve_f64 is None:
+        solve_f64 = groups == 1
+    out = torch.empty((groups, 10), dtype=torch.float64, device=dev)
+    params = torch.empty((groups, 3, 6), dtype=torch.float32, device=dev) if want_params else None
+    if x.numel() == 0:
+        out.zero_()
+        return (out, params) if want_params else out
+    need = lib.fqb200_clip_error_workspace_bytes(outer, groups, inner, int(bool(channels_last)))
+    if need == 0:
+        L.check(L.ERR_INVALID)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev), _Timed("E", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)):
+        L.check(lib.fqb200_clip_error(x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(),
+                                      int(num_bits), int(bool(positive)), int(bool(bit_alloc)), int(bool(solve_f64)),
+                                      out.data_ptr(), params.data_ptr() if params is not None else None, ws.data_ptr(), need,
+                                      int(max_ctas), _stream_handle(dev)))
+    return (out, params) if want_params else out
 
 
 def add_relu_(a, b):

@@ -13,7 +13,10 @@ implementation can be used by the other:
 Collect mode is an offline, one-time pass.  The five statistics the quantizers consume in use mode (min, max, mean,
 b, std) come from ONE statistics-only launch of the fused kernel per hooked tensor; the diagnostic columns the
 reference also writes (kurtosis, mean_abs, std_pos) are computed with plain torch ops; the error columns
-(mse_*/cos_*) are NaN exactly as in the reference's own collect runs (it never passes quantized tensors there).
+(mse_*/cos_*) are NaN exactly as in the reference's own collect runs (it never passes quantized tensors there), unless
+the caller hands ``save_tensor_stats`` a ``ClipErrConfig``: then one ops.clip_error launch per hooked tensor fills them
+with the errors of the three candidates `-c mix` chooses between (lowp, gaus, laplace), each configured like the
+tensor's use-mode quantizer.
 With ``kld_threshold`` the per-tensor manager adds the ``kld_th`` column: the max over the samples of the KL-divergence
 threshold (ops.kld_threshold, three launches and one read-back per hooked tensor).
 
@@ -23,6 +26,7 @@ threshold (ops.kld_threshold, three launches and one read-back per hooked tensor
 
 Each hooked tensor costs one ops.sample_sumsq launch; the results stay on the device until ``__exit__``.
 """
+import collections
 import os
 import pickle
 import re
@@ -33,7 +37,7 @@ import torch
 
 from . import ops
 
-__all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "default_base_dir"]
+__all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "ClipErrConfig", "default_base_dir"]
 
 
 def default_base_dir():
@@ -47,6 +51,57 @@ def sorted_nicely(keys):
 
 
 _ERR_COLUMNS = ["mse_lowp", "mse_gaus", "mse_laplace", "cos_lowp", "cos_gaus", "cos_laplace"]
+
+# The use-mode quantizer of one call site, as far as the error candidates need it: its bit width, its positive range
+# (half_range / force_positive), whether it quantizes this tensor per channel (pcq_a on a 4-D tensor with H or W > 1 and
+# C > 1, int_quantizer.py:333, :343-344) and its bit allocation (per channel with num_bits <= 4 only; prior PRIOR_STD /
+# PRIOR_B).
+ClipErrConfig = collections.namedtuple("ClipErrConfig", "num_bits positive per_channel bit_alloc bit_alloc_prior "
+                                                        "bit_alloc_round bit_alloc_target")
+
+
+def _clip_sums(t, cfg, per_sample_channel):
+    """float64 ops.clip_error sums (columns as there) of the contiguous ``t`` for the candidates ``cfg`` describes:
+    [1, 10] over the whole tensor, or with ``per_sample_channel`` [N, C, 10] per (sample, channel) - the per-channel
+    manager needs the per-sample norms of the reference's cos_sim(dims=[-1, 0]).  The candidates' statistics are those
+    of the on-the-fly launch of that quantizer (per tensor: the whole tensor; per channel: each channel, with the bit
+    allocation's widths); a per-(sample, channel) launch gets that table repeated for every group."""
+    n = t.shape[0]
+    if cfg.per_channel:
+        c = t.shape[1]
+        hw = t.numel() // (n * c)
+        table = ops.fused(t, (n, c, hw), num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
+                          bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
+                          bit_alloc_target=cfg.bit_alloc_target, stats_only=True)
+    else:
+        table = ops.fused(t, (1, 1, t.numel()), stats_only=True)
+    if not per_sample_channel:
+        if cfg.per_channel:   # all channels' errors together (a per-channel quantizer with per-tensor statistics)
+            return _clip_sums(t, cfg, True).sum((0, 1)).view(1, -1)
+        return ops.clip_error(t, table, (1, 1, t.numel()), False, cfg.num_bits, cfg.positive, solve_f64=True)
+    c = t.shape[1]
+    hw = t.numel() // (n * c)
+    table = table.repeat(n, 1) if cfg.per_channel else table.expand(n * c, -1).contiguous()
+    sums = ops.clip_error(t, table, (1, n * c, hw), False, cfg.num_bits, cfg.positive, bit_alloc=cfg.bit_alloc,
+                          solve_f64=not cfg.per_channel)
+    return sums.view(n, c, 10)
+
+
+def _clip_errors(sums, count, per_channel):
+    """{mse_k, cos_k} float32 device tensors from _clip_sums: per tensor ([1, 10]) mse = sum (x - q)^2 / count and
+    cos = sum x q / (sqrt(sum x^2) sqrt(sum q^2)) (statistic_manager.py:83-103); per channel ([N, C, 10]) mse over the
+    channel's N * HW elements and the reference's cos_sim(dims=[-1, 0]): sum_n sum_hw x q /
+    (sqrt(sum_n sqrt(sum_hw x^2)) sqrt(sum_n sqrt(sum_hw q^2))) (statistic_manager_perchannel.py:80-100, utils/misc.py)."""
+    res = {}
+    for k, name in enumerate(ops.CLIP_ERROR_CANDIDATES):
+        if per_channel:
+            res["mse_" + name] = (sums[:, :, 1 + k].sum(0) / count).float()
+            res["cos_" + name] = (sums[:, :, 4 + k].sum(0) / (sums[:, :, 0].sqrt().sum(0).sqrt()
+                                                              * sums[:, :, 7 + k].sqrt().sum(0).sqrt())).float()
+        else:
+            res["mse_" + name] = (sums[:, 1 + k] / count).float()
+            res["cos_" + name] = (sums[:, 4 + k] / (sums[:, 0].sqrt() * sums[:, 7 + k].sqrt())).float()
+    return res
 
 
 class StatisticManager(object):
@@ -74,12 +129,17 @@ class StatisticManager(object):
             self.stats_df = pd.read_csv(path, index_col=0)
 
     # -- collect ---------------------------------------------------------------------------------------
-    def save_tensor_stats(self, tensor, tag, id, tensors_q=None, force_global_min_max=False):
-        """One row of statistics for this batch (statistic_manager.py:47-122)."""
+    def save_tensor_stats(self, tensor, tag, id, tensors_q=None, force_global_min_max=False, clip_err=None):
+        """One row of statistics for this batch (statistic_manager.py:47-122).  ``clip_err`` (a ClipErrConfig): fill the
+        mse_* / cos_* columns with the errors of the `-c mix` candidates configured like that (else they are NaN)."""
         t = tensor.detach().contiguous()
         n = t.shape[0]
         st = ops.fused(t, (1, 1, t.numel()), stats_only=True)[0]  # min max mean b std over the whole tensor
         glob = {"min": st[0], "max": st[1], "mean": st[2], "b": st[3], "std": st[4]}
+        err = None
+        if clip_err is not None and any(c in self.stats_names for c in _ERR_COLUMNS):
+            e = _clip_errors(_clip_sums(t, clip_err, False), float(t.numel()), False)
+            err = dict(zip(_ERR_COLUMNS, torch.cat([e[c] for c in _ERR_COLUMNS]).cpu().tolist()))   # one copy
         if self.batch_avg and not force_global_min_max:
             per = ops.fused(t, (1, n, t.numel() // n), stats_only=True)
             glob["min"], glob["max"] = per[:, 0].mean(), per[:, 1].mean()
@@ -96,6 +156,8 @@ class StatisticManager(object):
                 v = flat.numel()
             elif sn == "kld_th":
                 v = ops.kld_threshold(t)[0].max()   # the max of the per-sample thresholds (NaN propagates, as np.max)
+            elif err is not None:  # mse_* / cos_*
+                v = err[sn]
             else:  # mse_* / cos_*: the reference writes NaN when no quantized tensors are handed in
                 v = float("nan")
             row.append(float(v))
@@ -167,8 +229,10 @@ class StatisticManagerPerChannel(object):
             with open(path, "rb") as f:
                 self.stats = pickle.load(f)
 
-    def save_tensor_stats(self, tensor, tag, id, tensors_q=None, force_global_min_max=False):
-        """Per-channel rows for this batch (statistic_manager_perchannel.py:45-122); FC / 1x1 tensors are skipped."""
+    def save_tensor_stats(self, tensor, tag, id, tensors_q=None, force_global_min_max=False, clip_err=None):
+        """Per-channel rows for this batch (statistic_manager_perchannel.py:45-122); FC / 1x1 tensors are skipped.
+        ``clip_err`` (a ClipErrConfig): fill the mse_* / cos_* rows, when the manager has those columns (collect_err), with
+        the per-channel errors of the `-c mix` candidates configured like that."""
         if tensor.dim() < 3 or (tensor.shape[2] == 1 and tensor.shape[3] == 1):
             return
         t = tensor.detach().contiguous()
@@ -176,6 +240,8 @@ class StatisticManagerPerChannel(object):
         hw = t.numel() // (n * c)
         st = ops.fused(t, (n, c, hw), stats_only=True)  # [C, 12]: min max mean b std ...
         vals = {"min": st[:, 0], "max": st[:, 1], "mean": st[:, 2], "b": st[:, 3], "std": st[:, 4]}
+        if clip_err is not None and any(s in self.stats_names for s in _ERR_COLUMNS):
+            vals.update(_clip_errors(_clip_sums(t, clip_err, True), float(n * hw), True))
         if not force_global_min_max:
             per = ops.fused(t, (1, n * c, hw), stats_only=True).view(n, c, -1)  # per (n, c)
             if self.batch_avg:
@@ -196,6 +262,9 @@ class StatisticManagerPerChannel(object):
             else:
                 continue  # mse_* / cos_* need quantized tensors: skipped like the reference does
             v = v.detach().cpu().numpy()
+            if sn.startswith("cos_"):   # statistic_manager_perchannel.py:113-115
+                v = np.nan_to_num(v)
+                v[v == 0] = 1.
             entry = self.stats.setdefault(id, {})
             entry[sn] = v if sn not in entry else np.vstack([entry[sn], v])
 

@@ -267,6 +267,28 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
 /* Workspace of fqb200_sample_sumsq in bytes (0 and fqb200_last_error() on bad arguments: rows < 0, row_len <= 0). */
 size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len);
 
+/*
+ * Clipping-error measurement (the mse_* / cos_* columns of `-sm collect`, statistic_manager.py:83-111): for every group g
+ * of x (layout as fqb200_desc: outer x groups x inner, NCHW order; or channels_last != 0: [outer][inner][groups] memory,
+ * groups % 4 == 0, 4 <= groups <= 2048) and the three candidate quantizers of get_alpha(clip_type='mix')
+ * (int_quantizer.py:310-323; k = 0 lowp: alpha = (max - min) / 2, 1 gaus, 2 laplace), out[g * 10 + j] =
+ *   j = 0: sum x^2;  j = 1 + k: sum (x - q_k)^2;  j = 4 + k: sum x * q_k;  j = 7 + k: sum q_k^2     (float64)
+ * where q_k is the torch leaf (FQB200_LEAF_TORCH) with candidate k's parameters, solved on the device from `stats`, the
+ * [groups][FQB200_STATS_STRIDE] table of a stats_only fqb200_fused launch on the same x: alpha2DeltaOffset in float64
+ * when solve_f64 (per tensor) else fp32, the positive range when `positive`, num_bits (1..8) or, with bit_alloc
+ * (num_bits <= 4), the table's allocated widths (column 7) - exactly the parameters the on-the-fly quantizer of each clip
+ * type computes from that table.  out_params (optional, [groups][3][6] floats): per candidate delta, offset, bits, scale,
+ * zero point, qmax.  An NCHW group with outer > 1 must hold fewer than 2^32 elements.  One read of x (4 B/element) and a
+ * small second launch on `stream`; nothing else is written, no host synchronisation.  Work units and summation order
+ * are fixed (no atomics on values): the bits do not depend on the run or on max_ctas (0: the default grid, else at most
+ * that many CTAs).  The workspace (fqb200_clip_error_workspace_bytes, 16-byte aligned) is private to the call.
+ */
+int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last, const float* stats,
+                      int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, double* out, float* out_params,
+                      void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream);
+/* Workspace of fqb200_clip_error in bytes (0 and fqb200_last_error() on a layout it does not take). */
+size_t fqb200_clip_error_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last);
+
 #ifdef __cplusplus
 }
 #endif
