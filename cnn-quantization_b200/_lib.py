@@ -21,7 +21,8 @@ SYMBOLS = ("fqb200_abi_version", "fqb200_last_error", "fqb200_resident_ctas", "f
            "fqb200_selftest_division", "fqb200_workspace_bytes", "fqb200_workspace_init", "fqb200_float2gemmlowp",
            "fqb200_quantize1", "fqb200_quantize1_bca", "fqb200_fused", "fqb200_add_relu", "fqb200_maxpool2d_nhwc",
            "fqb200_kld_threshold", "fqb200_kld_workspace_bytes", "fqb200_sample_sumsq",
-           "fqb200_sample_sumsq_workspace_bytes", "fqb200_clip_error", "fqb200_clip_error_workspace_bytes")
+           "fqb200_sample_sumsq_workspace_bytes", "fqb200_clip_error", "fqb200_clip_error_workspace_bytes",
+           "fqb200_kmeans1d", "fqb200_kmeans1d_workspace_bytes")
 ABI_VERSION = 3
 
 
@@ -105,6 +106,11 @@ def load():
     lib.fqb200_clip_error.argtypes = [vp, i64, i64, i64, i32, vp, i32, i32, i32, i32, vp, vp, vp, ctypes.c_size_t, i32, vp]
     lib.fqb200_clip_error_workspace_bytes.restype = ctypes.c_size_t
     lib.fqb200_clip_error_workspace_bytes.argtypes = [i64, i64, i64, i32]
+    lib.fqb200_kmeans1d.restype = i32
+    lib.fqb200_kmeans1d.argtypes = [vp, i64, i32, i64, vp, i32, vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_size_t,
+                                    i32, vp]
+    lib.fqb200_kmeans1d_workspace_bytes.restype = ctypes.c_size_t
+    lib.fqb200_kmeans1d_workspace_bytes.argtypes = [i64, i32]
     lib.fqb200_plan_info.restype = i32
     lib.fqb200_plan_info.argtypes = [ctypes.POINTER(Desc), ctypes.POINTER(ctypes.c_int64)]
     if lib.fqb200_abi_version() != ABI_VERSION:

@@ -1101,6 +1101,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_kld.cuh"
 #include "fq_measure.cuh"
 #include "fq_cliperr.cuh"
+#include "fq_kmeans.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1655,6 +1656,49 @@ unsigned long long cliperr_units_per_group(int64_t outer, int64_t inner, int cha
 }
 size_t cliperr_workspace(int64_t outer, int64_t groups, int64_t inner, int channels_last) {
   return static_cast<size_t>(groups) * static_cast<size_t>(cliperr_units_per_group(outer, inner, channels_last)) * fqb::kCeSums * 8;
+}
+
+// k-means workspace (fq_kmeans.cuh): barrier words, control block, per-block / per-superblock column sums, Lloyd unit
+// partials, relocation candidates.  Fills A's pointers when base != nullptr.
+size_t kmeans_carve(char* base, unsigned long long n, int k, fqb::KmArgs* A) {
+  const unsigned long long nb = (n + fqb::kKmBlk - 1) / fqb::kKmBlk, nsb = (nb + fqb::kKmSuper - 1) / fqb::kKmSuper;
+  const unsigned long long per = fqb::kWarps * ((nb + fqb::kWarps * fqb::kKmMaxUnits - 1) / (fqb::kWarps * fqb::kKmMaxUnits));
+  const unsigned long long units = (nb + per - 1) / per;
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    char* p = base ? base + off : nullptr;
+    off = align_up(off + bytes, 256);
+    return p;
+  };
+  char* sync = take(sizeof(fqb::GridSync));
+  char* ctrl = take(sizeof(fqb::KmCtrl));
+  char* col = take(static_cast<size_t>(fqb::kKmMaxT) * nb * 8);
+  char* sup = take(static_cast<size_t>(fqb::kKmMaxT) * nsb * 8);
+  char* usum = take(static_cast<size_t>(units) * k * 8);
+  char* ucnt = take(static_cast<size_t>(units) * k * 4);
+  char* rbd = take(static_cast<size_t>(nb) * 8);
+  char* rbi = take(static_cast<size_t>(nb) * 8);
+  char* far = take(static_cast<size_t>(k) * 8);
+  if (A) {
+    A->n = n; A->nb = nb; A->nsb = nsb; A->k = k;
+    A->unit_blocks = per; A->units = units;
+    A->sync = reinterpret_cast<fqb::GridSync*>(sync);
+    A->ctrl = reinterpret_cast<fqb::KmCtrl*>(ctrl);
+    A->col = reinterpret_cast<double*>(col);
+    A->sup = reinterpret_cast<double*>(sup);
+    A->usum = reinterpret_cast<double*>(usum);
+    A->ucnt = reinterpret_cast<unsigned*>(ucnt);
+    A->rbd = reinterpret_cast<double*>(rbd);
+    A->rbi = reinterpret_cast<long long*>(rbi);
+    A->far = reinterpret_cast<long long*>(far);
+  }
+  return off;
+}
+size_t kmeans_smem(int k) {
+  const size_t stage = static_cast<size_t>(fqb::kKmMaxT) * fqb::kKmBlk * 8;
+  const size_t acc = static_cast<size_t>(fqb::kWarps) * k * 12;
+  const size_t tot = static_cast<size_t>(fqb::kThreads) * 16;
+  return stage > acc ? (stage > tot ? stage : tot) : (acc > tot ? acc : tot);
 }
 
 // workspace layout; returns total bytes, fills pointers when base != nullptr.  Partials: one slot per unit.
@@ -2398,6 +2442,85 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
   fqb::fq_cliperr_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCeThreads, 0, st>>>(A);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch clipping-error kernels: %s", cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+// the requests fqb200_kmeans1d takes (argument errors as a message, nullptr when they are fine)
+static const char* kmeans_bad_args(int64_t n, int32_t k) {
+  if (k < 2 || k > fqb::kKmMaxK || (k & (k - 1))) return "k must be a power of two, 2 .. 256%s";
+  if (n < k) return "n must be >= k (scikit-learn raises for fewer samples than clusters)%s";
+  if (n >= (1ll << 40)) return "n must be < 2^40%s";
+  return nullptr;
+}
+
+size_t fqb200_kmeans1d_workspace_bytes(int64_t n, int32_t k) {
+  g_err[0] = 0;
+  const char* bad = kmeans_bad_args(n, k);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  return kmeans_carve(nullptr, static_cast<unsigned long long>(n), k, nullptr);
+}
+
+int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_id, const double* draws, int32_t n_trials,
+                    const double* init, int32_t task, int64_t rows, uint8_t* out_labels, float* out_centres,
+                    double* out_inertia, int32_t* out_n_iter, int64_t* out_init_ids, float* out, float* out_bcorr,
+                    void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
+  const int k = 1 << num_bits;
+  const char* bad = kmeans_bad_args(n, k);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!in || !out_labels || !out_centres || !out_inertia || !out_n_iter) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (task != FQB200_KMEANS_NONE && task != FQB200_KMEANS_QUANTIZE && task != FQB200_KMEANS_CLIP)
+    return fail(FQB200_ERR_INVALID, "task must be FQB200_KMEANS_NONE, _QUANTIZE or _CLIP%s");
+  if (task != FQB200_KMEANS_NONE && !out) return fail(FQB200_ERR_INVALID, "a task needs `out`%s");
+  if (rows < 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0%s");
+  if (rows > 0 && (task == FQB200_KMEANS_NONE || !out_bcorr || n % rows != 0))
+    return fail(FQB200_ERR_INVALID, "rows > 0 needs a task, out_bcorr and n %% rows == 0%s");
+  if (!init) {
+    if (!draws) return fail(FQB200_ERR_INVALID, "k-means++ needs the draws (or pass init)%s");
+    if (first_id < 0 || first_id >= n) return fail(FQB200_ERR_INVALID, "first_id must be in 0 .. n - 1%s");
+    if (n_trials < 1 || n_trials > 7) return fail(FQB200_ERR_INVALID, "n_trials must be in 1..7%s");
+  }
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  fqb::KmArgs A;
+  memset(&A, 0, sizeof(A));
+  const size_t need = kmeans_carve(static_cast<char*>(workspace), static_cast<unsigned long long>(n), k, &A);
+  if (!workspace || workspace_bytes < need || !aligned16(workspace))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_kmeans1d_workspace_bytes() or not 16-byte aligned%s");
+  DeviceInfo* di = nullptr;
+  int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  A.in = in;
+  A.T = init ? 1 : n_trials;
+  A.task = task;
+  A.given = init ? 1 : 0;
+  A.first_id = init ? 0 : first_id;
+  A.draws = draws;
+  A.init = init;
+  A.rows = static_cast<unsigned long long>(rows);
+  A.labels = out_labels;
+  A.centres = out_centres;
+  A.inertia = out_inertia;
+  A.n_iter = out_n_iter;
+  A.init_ids = init ? nullptr : reinterpret_cast<long long*>(out_init_ids);
+  A.out = out;
+  A.out_bcorr = out_bcorr;
+  const void* fn = reinterpret_cast<const void*>(fqb::fq_kmeans_kernel);
+  const size_t smem = kmeans_smem(k);
+  int per_sm = 0;
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, fqb::kThreads, smem);
+  if (e != cudaSuccess || per_sm < 1) return fail(FQB200_ERR_CUDA, "k-means kernel setup: %s", cudaGetErrorString(e));
+  const long long resident = static_cast<long long>(di->sms) * per_sm;
+  const long long grid = max_ctas && max_ctas < resident ? max_ctas : resident;
+  // barrier words and control block start at zero
+  e = cudaMemsetAsync(workspace, 0, reinterpret_cast<char*>(A.col) - static_cast<char*>(workspace), st);
+  if (e == cudaSuccess && init && out_init_ids) e = cudaMemsetAsync(out_init_ids, 0xff, static_cast<size_t>(k) * 8, st);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaMemsetAsync: %s", cudaGetErrorString(e));
+  void* args[] = {&A};
+  e = cudaLaunchCooperativeKernel(fn, dim3(static_cast<unsigned>(grid)), dim3(fqb::kThreads), args, smem, st);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_kmeans_kernel: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
 

@@ -1,7 +1,9 @@
 """Tensor-level wrappers over the C ABI: device pointers and the current stream come from torch, the
 arithmetic all happens in libfqb200.so.  Nothing here synchronises with the host."""
+import collections
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -22,7 +24,8 @@ def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
-    (ops.sample_sumsq) and 'E' the clipping-error measurement (ops.clip_error), which quantize nothing."""
+    (ops.sample_sumsq), 'E' the clipping-error measurement (ops.clip_error) and 'C' the k-means clustering of a weight
+    tensor (ops.kmeans1d), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -513,6 +516,87 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
                                       out.data_ptr(), params.data_ptr() if params is not None else None, ws.data_ptr(), need,
                                       int(max_ctas), _stream_handle(dev)))
     return (out, params) if want_params else out
+
+
+KMeans1d = collections.namedtuple("KMeans1d", "labels centres inertia n_iter init_ids out out_bcorr")
+KMEANS_TASKS = {None: 0, "quantize": 1, "clip": 2}
+
+
+def kmeans_trials(k):
+    """scikit-learn's number of k-means++ local trials: 2 + int(log k)."""
+    return 2 + int(np.log(k))
+
+
+def kmeans_draws(n, k, seed):
+    """The random draws of scikit-learn's k-means++ (_kmeans_plusplus) on ``np.random.RandomState(seed)``, in its order: the
+    first centre ``choice(n, p=w / w.sum())`` with float32 unit weights, then ``uniform(size=n_local_trials)`` for every
+    further centre.  They do not depend on the data.  Returns (first index, float64 [k - 1, n_local_trials])."""
+    rs = np.random.RandomState(seed)
+    w = np.ones(n, dtype=np.float32)
+    first = int(rs.choice(n, p=w / w.sum()))
+    del w
+    t = kmeans_trials(k)
+    u = np.stack([rs.uniform(size=t) for _ in range(k - 1)]) if k > 1 else np.zeros((0, t))
+    return first, u
+
+
+def kmeans1d(x, num_bits, seed=0, task=None, init=None, rows=None, max_ctas=0):
+    """C ABI fqb200_kmeans1d: scikit-learn's ``KMeans(n_clusters=2**num_bits, random_state=seed).fit`` on the values of the
+    dense tensor ``x`` in memory order (kmeans_quantization.py:14-30), in one launch.  ``task`` 'quantize' also returns
+    ``out`` = each value replaced by its centre, 'clip' returns ``x`` clipped to [min, max] of the centres; ``rows`` (with a
+    task) adds ``out_bcorr``, the per-output-channel bias correction of kmeans_quantization.py:86-88 over ``rows`` rows
+    (float64 row means, rounded to fp32 once).  ``init``: initial centres (k values in the data's units, scikit-learn's
+    ``init=``) instead of k-means++.  Returns a ``KMeans1d`` of device tensors: labels (uint8, x's shape), centres (float32
+    [k], centre + mean like ``cluster_centers_``), inertia (float64 scalar), n_iter (int32 scalar), init_ids (int64 [k], the
+    k-means++ sample indices; -1 with ``init``), out and out_bcorr (x's shape and strides, or None).  Non-finite input raises
+    ValueError, as scikit-learn does (one host synchronisation for that check); otherwise the launch does not synchronise.
+    Deterministic: the bits depend neither on the run nor on ``max_ctas``.  Recorded in the launch profile under mode
+    'C'."""
+    _require_cuda_f32(x, "tensor")
+    if task not in KMEANS_TASKS:
+        raise ValueError("task must be None, 'quantize' or 'clip'")
+    num_bits = int(num_bits)
+    if not 1 <= num_bits <= 8:
+        raise ValueError("num_bits must be in 1..8")
+    k = 1 << num_bits
+    if not dense(x):
+        x = x.contiguous()
+    n = x.numel()
+    if n < k:
+        raise ValueError("n_samples=%d should be >= n_clusters=%d." % (n, k))
+    if not bool(torch.isfinite(x).all()):
+        raise ValueError("Input contains NaN or infinity.")
+    rows = int(rows or 0)
+    if rows and (task is None or n % rows):
+        raise ValueError("rows needs a task and must divide the number of elements")
+    lib = L.load()
+    dev = x.device
+    labels = torch.empty_like(x, dtype=torch.uint8)
+    centres = torch.empty(k, dtype=torch.float32, device=dev)
+    inertia = torch.empty((), dtype=torch.float64, device=dev)
+    n_iter = torch.empty((), dtype=torch.int32, device=dev)
+    init_ids = torch.empty(k, dtype=torch.int64, device=dev)
+    out = torch.empty_like(x) if task else None
+    out_bcorr = torch.empty_like(x) if rows else None
+    first, draws, init_t = 0, None, None
+    if init is None:
+        first, u = kmeans_draws(n, k, seed)
+        draws = torch.from_numpy(np.ascontiguousarray(u, dtype=np.float64)).to(dev)
+    else:
+        init_t = torch.as_tensor(init, dtype=torch.float64).reshape(-1).to(dev).contiguous()
+        if init_t.numel() != k:
+            raise ValueError("init must hold %d centres" % k)
+    need = lib.fqb200_kmeans1d_workspace_bytes(n, k)
+    if need == 0:
+        L.check(L.ERR_INVALID)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+    with torch.cuda.device(dev), _Timed("C", n, 4, "%d k=%d" % (n, k)):
+        L.check(lib.fqb200_kmeans1d(x.data_ptr(), n, num_bits, first, ptr(draws), kmeans_trials(k), ptr(init_t),
+                                    KMEANS_TASKS[task], rows, labels.data_ptr(), centres.data_ptr(), inertia.data_ptr(),
+                                    n_iter.data_ptr(), init_ids.data_ptr(), ptr(out), ptr(out_bcorr), ws.data_ptr(), need,
+                                    int(max_ctas), _stream_handle(dev)))
+    return KMeans1d(labels, centres, inertia, n_iter, init_ids, out, out_bcorr)
 
 
 def add_relu_(a, b):

@@ -289,6 +289,36 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
 /* Workspace of fqb200_clip_error in bytes (0 and fqb200_last_error() on a layout it does not take). */
 size_t fqb200_clip_error_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last);
 
+/*
+ * 1-D k-means quantization of one weight tensor (pytorch_quantizer/quantization/kmeans_quantization.py:14-30): scikit-learn
+ * 1.9's KMeans(n_clusters=k, random_state=seed).fit on the n floats of `in` in memory order (k = 2^num_bits, num_bits 1..8,
+ * k <= n < 2^40): the data centred on its mean, one k-means++ init, Lloyd with max_iter 300 and tol = var(in) * 1e-4,
+ * empty clusters relocated to the farthest points, all in float64 with fixed summation orders (fq_kmeans.cuh).
+ *   k-means++: first_id (0 .. n - 1) is the first centre and draws[(c - 1) * n_trials + t] (device, float64) the uniforms of
+ *   step c = 1 .. k - 1, trial t (n_trials = 2 + int(log k)) - the host's np.random.RandomState(seed).choice / .uniform
+ *   calls in scikit-learn's order; the draws do not depend on the data.  init != NULL (device, k float64 centres in the
+ *   data's units, scikit-learn's init= array) replaces k-means++; first_id, draws and n_trials are then ignored.
+ * Writes out_labels[n] (nearest centre, ties to the lowest index), out_centres[k] (float32 of centre + mean, like
+ * cluster_centers_), out_inertia (float64, about the centred data), out_n_iter, and out_init_ids[k] (the k-means++ sample
+ * indices; -1 with init; may be NULL).  task FQB200_KMEANS_QUANTIZE writes out[i] = out_centres[label[i]], FQB200_KMEANS_CLIP
+ * writes in clipped to [min, max] of out_centres, FQB200_KMEANS_NONE writes no tensor (out may be NULL).  rows > 0 (with a
+ * task; n % rows == 0) also writes out_bcorr = fp32(out - (mean_row(out) - mean_row(in))) over `rows` rows of n / rows
+ * (kmeans_quantization.py:86-88; the row means in float64).  `out` and `out_bcorr` must not alias `in`.
+ * One cooperative launch on `stream` (and two small memsets); no host synchronisation.  No atomics on values: the bits do not
+ * depend on the run or on max_ctas (0: every resident CTA, else at most that many).  The workspace
+ * (fqb200_kmeans1d_workspace_bytes, 16-byte aligned) is private to the call; it needs no initialisation.
+ */
+#define FQB200_KMEANS_NONE 0
+#define FQB200_KMEANS_QUANTIZE 1
+#define FQB200_KMEANS_CLIP 2
+int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_id, const double* draws, int32_t n_trials,
+                    const double* init, int32_t task, int64_t rows, uint8_t* out_labels, float* out_centres,
+                    double* out_inertia, int32_t* out_n_iter, int64_t* out_init_ids, float* out, float* out_bcorr,
+                    void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream);
+/* Workspace of fqb200_kmeans1d in bytes for n elements and k clusters (0 and fqb200_last_error() when k is not a power of
+ * two in 2 .. 256 or n < k). */
+size_t fqb200_kmeans1d_workspace_bytes(int64_t n, int32_t k);
+
 #ifdef __cplusplus
 }
 #endif
