@@ -1257,8 +1257,8 @@ namespace {
 
 thread_local char g_err[512] = "";
 
-int fail(int code, const char* fmt, const char* detail = "") {
-  snprintf(g_err, sizeof(g_err), fmt, detail);
+int fail(int code, const char* fmt, const char* detail = "", const char* detail2 = "") {
+  snprintf(g_err, sizeof(g_err), fmt, detail, detail2);
   return code;
 }
 
@@ -1771,16 +1771,199 @@ int check_desc(const fqb200_desc* d) {
   return FQB200_OK;
 }
 
-// what the channels-last kernel can take (everything else with channels_last set is an error: the caller re-lays out)
-bool cl_supported(const fqb200_desc* d) {
-  return d->scope == FQB200_SCOPE_GROUP && d->leaf != FQB200_LEAF_COMPILED && !d->bias_corr && !d->var_corr && d->bias_period <= 0 &&
-         flat_eligible(d->groups);
+// Widest pooling tile (pixels) whose row pieces fit a ring stage, 0 if none.  2x2: a tile is 2 rows x wt input pixels,
+// two row pieces in the two halves of a stage, (wt / 2) * cv output vectors.  3x3: a tile is 1 output row x wt output
+// pixels, three row pieces of 2 * wt + 1 input pixels in three regions of a stage.
+unsigned pool_tile_width(int kind, int64_t w, const fqb::FlatGeo& f) {
+  const unsigned cv = f.cv, stage_v = fqb::kStageVec * fqb::kConsumers;
+  if (kind == 2) {
+    for (int64_t cand = w; cand >= 2; cand -= 2)
+      if (w % cand == 0 && static_cast<uint64_t>(cand) * cv <= stage_v / 2u && static_cast<uint64_t>(cand / 2) * cv <= f.stride)
+        return static_cast<unsigned>(cand);
+  } else {
+    const int64_t ow = w / 2;
+    for (int64_t cand = ow; cand >= 1; --cand)
+      if (ow % cand == 0 && 3ull * static_cast<uint64_t>(2 * cand + 1) * cv <= stage_v && static_cast<uint64_t>(cand) * cv <= f.stride)
+        return static_cast<unsigned>(cand);
+  }
+  return 0;
 }
-// phase S2 (sum |x - mean|) of the channels-last kernel: only where the Laplace b is consumed
-bool cl_needs_b(const fqb200_desc* d) {
-  const bool alloc = d->bit_alloc && d->num_bits <= 4 && d->leaf != FQB200_LEAF_MIDTREAD;
-  return d->range_mode == FQB200_RANGE_LAPLACE || (d->leaf == FQB200_LEAF_MIDTREAD && d->mt_clip) ||
-         (alloc && d->bit_alloc_prior == FQB200_PRIOR_B) || d->stats_only || d->out_stats != nullptr;
+
+// One fqb200_fused launch: route, geometry, kernel and its arguments, all but in / out and the workspace pointers.
+struct FusedPlan {
+  Plan pl;                    // mode 2: channels-last flat stream, 3: rows, 4 / 1 / 8: fq_fused_kernel
+  fqb::FusedArgs A;
+  uint64_t slots;             // per-unit partial slots in the workspace
+  size_t workspace;           // bytes the launch needs (0: none)
+  const void* kernel;
+  unsigned block;
+  size_t smem;
+  bool coop;
+  const char* name;
+};
+
+// The single place where a fused descriptor's route is decided and refused.  `d` passed check_desc; `can_vec`: in / out
+// are 16-byte aligned; `r` holds the resident-CTA counts the grids are sized for.  No CUDA calls.
+int plan_fused(const fqb200_desc* d, bool can_vec, const DeviceInfo& r, FusedPlan* fp) {
+  memset(fp, 0, sizeof(*fp));
+  Plan& pl = fp->pl;
+  fqb::FusedArgs& A = fp->A;
+  if (d->outer <= 0 || d->groups <= 0 || d->inner <= 0) return fail(FQB200_ERR_INVALID, "non-positive tensor extent%s");
+  if (d->bias && d->bias_period == 0 && d->scope == FQB200_SCOPE_GROUP_MEAN)
+    return fail(FQB200_ERR_UNSUPPORTED, "a per-group bias needs groups = channels (scope GROUP or TENSOR); use bias_period%s");
+  const bool given = d->range_mode == FQB200_RANGE_GIVEN;
+  int rc;
+  if (d->channels_last) {
+    // what the channels-last kernel can take (everything else with channels_last set is an error: the caller re-lays out)
+    if (!can_vec || d->scope != FQB200_SCOPE_GROUP || d->leaf == FQB200_LEAF_COMPILED || d->bias_corr || d->var_corr ||
+        d->bias_period > 0 || !flat_eligible(d->groups))
+      return fail(FQB200_ERR_UNSUPPORTED, "channels_last: per-channel torch / mid-tread leaves on 16-byte aligned tensors, C %% 4 == 0, C <= 2048%s");
+    rc = make_plan_flat(static_cast<uint64_t>(d->outer) * d->groups * d->inner, d->groups,
+                        given ? r.resident_cl[0] * 2 : r.resident_cl[d->out_hist ? 1 : 0], &pl);
+  } else if (rows_supported(d, can_vec)) {
+    rc = make_plan_rows(static_cast<uint64_t>(d->groups), static_cast<uint64_t>(d->inner), d->bias ? -d->bias_period : 0,
+                        r.resident_rows, &pl, &A.rows);
+  } else if (d->bias && d->bias_period < 0) {
+    return fail(FQB200_ERR_UNSUPPORTED, "a channel-fastest bias (bias_period < 0) needs the per-sample / per-tensor min-max layout%s");
+  } else {
+    rc = make_plan(d->outer, d->groups, d->inner, can_vec, !(d->bias_corr || d->var_corr), r.resident, &pl);
+  }
+  if (rc != FQB200_OK) return rc;
+  if ((d->residual_stats || d->residual_bias) && !d->residual)
+    return fail(FQB200_ERR_INVALID, "residual_stats / residual_bias without a residual%s");
+  if (d->residual_bias && !d->residual_stats)
+    return fail(FQB200_ERR_INVALID, "residual_bias needs residual_stats (a bias on a plain addend can be folded by the caller)%s");
+  if (d->residual && ((!d->channels_last && pl.mode != 3) || d->stats_only || !aligned16(d->residual)))
+    return fail(FQB200_ERR_UNSUPPORTED, "residual: channels-last or per-sample / per-tensor min-max apply launches, 16-byte aligned%s");
+  if (d->pool) {
+    // channels-last per-channel launches, or the per-sample / per-tensor min-max launches (rows = samples) on channels-last
+    // memory, which know the channel count from their channel-fastest bias
+    const bool rows_cl = pl.mode == 3 && d->bias && d->bias_period < 0;
+    if ((d->pool != 2 && d->pool != 3) || !(d->channels_last || rows_cl) || d->stats_only || d->residual || d->out_hist || !d->pool_out ||
+        !aligned16(d->pool_out))
+      return fail(FQB200_ERR_UNSUPPORTED, "pool: 2 (2x2 stride 2) or 3 (3x3 stride 2 padding 1) on channels-last apply launches without residual / histogram, 16-byte aligned pool_out%s");
+    const int64_t h = d->pool_h, w = d->pool_w;
+    const int64_t hw = rows_cl ? d->inner / -d->bias_period : d->inner;
+    const int64_t images = rows_cl ? d->groups : d->outer;
+    if (h < 2 || w < 2 || w % 2 != 0 || h * w != hw || (d->pool == 3 && h % 2 != 0))
+      return fail(FQB200_ERR_UNSUPPORTED, "pool: pool_h * pool_w must be H * W of the tensor, W even (3x3: H even too)%s");
+    const unsigned wt = pool_tile_width(d->pool, w, pl.flat);
+    if (!wt) return fail(FQB200_ERR_UNSUPPORTED, "pool: no tile width fits%s");
+    const int64_t tiles_per_row = (d->pool == 2 ? w : w / 2) / wt;
+    const uint64_t tiles = static_cast<uint64_t>(images) * static_cast<uint64_t>(h / 2) * static_cast<uint64_t>(tiles_per_row);
+    if (tiles >= 0xfffffff0ull) return fail(FQB200_ERR_UNSUPPORTED, "pool: too many tiles%s");
+    uint64_t unit_tiles = tiles / (kUnitsPerCta * static_cast<uint64_t>(pl.grid));
+    if (unit_tiles < 2) unit_tiles = 2;
+    if (unit_tiles > 64) unit_tiles = 64;
+    A.pool.h = static_cast<unsigned>(h);
+    A.pool.w = static_cast<unsigned>(w);
+    A.pool.wt = wt;
+    A.pool.tiles_per_row = static_cast<unsigned>(tiles_per_row);
+    A.pool.row_pairs = static_cast<unsigned>(h / 2);
+    A.pool.tiles = static_cast<unsigned>(tiles);
+    A.pool.unit_tiles = static_cast<unsigned>(unit_tiles);
+    A.pool.units = static_cast<unsigned>((tiles + unit_tiles - 1) / unit_tiles);
+    A.pool.ow = static_cast<unsigned>(w / 2);
+    A.pool.kind = static_cast<unsigned>(d->pool);
+    A.pool_out = d->pool_out;
+  }
+  A.hist_bins = d->out_hist ? (d->hist_bins > 0 ? d->hist_bins : 256) : 0;
+  if (d->out_hist && d->leaf != FQB200_LEAF_TORCH && !d->channels_last)
+    return fail(FQB200_ERR_UNSUPPORTED, "out_hist: torch leaf, or the mid-tread leaf on channels-last tensors%s");
+  if (d->out_hist && (A.hist_bins > static_cast<int>(fqb::kHistWords) || (!d->channels_last && A.hist_bins != 256)))
+    return fail(FQB200_ERR_UNSUPPORTED, "hist_bins: 256 (default), up to 8192 on channels-last tensors%s");
+  A.geo = pl.geo;
+  A.flat = pl.flat;
+  A.scope = d->scope;
+  A.range_mode = d->range_mode;
+  A.leaf = d->leaf;
+  A.num_bits = d->num_bits;
+  A.positive = d->positive;
+  A.solve_f64 = d->solve_f64;
+  A.clip_k = d->clip_k;
+  A.bit_alloc = d->bit_alloc;
+  A.prior = d->bit_alloc_prior;
+  A.ba_round = d->bit_alloc_round;
+  A.ba_target = d->bit_alloc_target;
+  A.mt_target = d->mt_target;
+  A.mt_clip = d->mt_clip;
+  A.bias_corr = d->bias_corr;
+  A.var_corr = d->var_corr;
+  A.stats_only = d->stats_only;
+  A.relu_passthrough = d->relu_passthrough;
+  A.residual = d->residual;
+  A.residual_relu = d->residual_relu;
+  A.residual_stats = d->residual_stats;
+  A.residual_bias = d->residual_bias;
+  A.out_stats = d->out_stats;
+  A.bias = d->bias;
+  A.hist = d->out_hist;
+  A.hist_offset = d->hist_offset;
+  A.hist_clamped = d->out_hist_clamped;
+  A.dbg = d->debug_stamps;
+  fp->block = fqb::kBulkThreads;
+  fp->coop = !given;
+  if (given) {  // no statistics, no barrier: no workspace
+    A.g_delta = d->given_delta;
+    A.g_offset = d->given_offset;
+    A.g_bits = d->given_bits;
+    A.given_per_group = 1;
+    fp->kernel = reinterpret_cast<const void*>(fqb::fq_cl_given_fused_kernel);
+    fp->smem = cl_given_smem();
+    fp->name = "fq_cl_given_fused_kernel";
+    return FQB200_OK;
+  }
+  if (pl.mode == 3) {
+    if (d->scope == FQB200_SCOPE_GROUP) A.scope = FQB200_SCOPE_TENSOR;  // one row
+    A.n_per_group = static_cast<double>(d->inner);
+    fp->kernel = reinterpret_cast<const void*>(fqb::fq_rows_kernel);
+    fp->smem = cl_given_smem();
+    fp->name = "fq_rows_kernel";
+  } else {
+    if (d->bias && d->bias_period > 0) {
+      // bias indexed by the channel inside the row: needs whole vectors per channel and an exact magic division
+      const uint64_t pv = static_cast<uint64_t>(d->bias_period) / pl.vec;
+      if (pl.mode != 4 || d->leaf != FQB200_LEAF_COMPILED || d->range_mode != FQB200_RANGE_MINMAX || d->bias_corr || d->var_corr ||
+          d->stats_only || d->bias_period % pl.vec != 0 || d->inner % d->bias_period != 0 || pv == 0 ||
+          static_cast<uint64_t>(pl.geo.inner_v) * pv >= (1ull << 40) || pl.geo.inner_v >= (1u << 24))
+        return fail(FQB200_ERR_UNSUPPORTED, "bias_period does not fit this layout%s");
+      A.bias_magic = ((1ull << 40) + pv - 1) / pv;
+    }
+    A.inner = static_cast<unsigned>(d->inner);
+    A.n_per_group = static_cast<double>(d->outer) * static_cast<double>(d->inner);
+    const bool alloc = d->bit_alloc && d->num_bits <= 4 && d->scope == FQB200_SCOPE_GROUP && d->leaf != FQB200_LEAF_MIDTREAD;
+    if (pl.mode == 2) {
+      // replicas of the per-channel accumulators: CTA b adds into replica b % rep (same-address atomics serialise in L2)
+      const unsigned rep = fqb::kMaxNhwcChannels / static_cast<unsigned>(d->groups);
+      A.nhwc_rep = rep < 1u ? 1u : (rep > 8u ? 8u : rep);
+      // phase S2 (sum |x - mean|) of the channels-last kernel: only where the Laplace b is consumed
+      A.need_dev = d->range_mode == FQB200_RANGE_LAPLACE || (d->leaf == FQB200_LEAF_MIDTREAD && d->mt_clip) ||
+                   (alloc && d->bit_alloc_prior == FQB200_PRIOR_B) || d->stats_only || d->out_stats != nullptr;
+      fp->kernel = cl_kernel_ptr(d->leaf, A.need_dev != 0, d->out_hist != nullptr);
+      fp->smem = cl_smem(d->out_hist != nullptr);
+      fp->name = "fq_cl_kernel";
+    } else {
+      A.nhwc_rep = 1;
+      A.need_dev = (d->range_mode != FQB200_RANGE_MINMAX) || alloc || d->var_corr || d->leaf == FQB200_LEAF_MIDTREAD || d->stats_only;
+      fp->slots = static_cast<uint64_t>(pl.geo.parts) * pl.geo.channels;  // the channels-last kernels use the accumulators
+      fp->kernel = A.bias_magic ? reinterpret_cast<const void*>(fqb::fq_fused_kernel<4, FQB200_LEAF_COMPILED, false, false, true>)
+                                : fused_kernel_ptr(pl.mode, d->leaf, A.need_dev != 0, d->bias_corr || d->var_corr);
+      fp->block = fqb::kThreads;
+      fp->smem = dyn_smem(pl.vec);
+      fp->name = "fq_fused_kernel";
+    }
+  }
+  fp->workspace = carve(nullptr, fp->slots, pl.geo.channels, nullptr);
+  return FQB200_OK;
+}
+
+// the resident-CTA counts plans are made for without a launch: the current device's, or an H100's when there is none
+DeviceInfo plan_residency() {
+  DeviceInfo* di = nullptr;
+  if (get_device(&di) == FQB200_OK) return *di;
+  DeviceInfo h;
+  h.resident = h.resident_cl[0] = h.resident_cl[1] = h.resident_rows = kAssumedSms * fqb::kCtasPerSm;
+  return h;
 }
 
 }  // namespace
@@ -1799,20 +1982,16 @@ int fqb200_resident_ctas(void) {
 
 size_t fqb200_workspace_bytes(const fqb200_desc* d) {
   if (check_desc(d) != FQB200_OK) return 0;
-  if (d->outer <= 0 || d->groups <= 0 || d->inner <= 0) return 256;
-  if (d->range_mode == FQB200_RANGE_GIVEN) return 256;  // not used by the launch; non-zero = "descriptor accepted"
-  int resident = kAssumedSms * fqb::kCtasPerSm;  // without a device: plan for an H100
-  DeviceInfo* di = nullptr;
-  if (get_device(&di) == FQB200_OK) resident = di->resident;
-  if (d->channels_last) return carve(nullptr, 0, static_cast<uint64_t>(d->groups), nullptr);
-  Plan a, b, c;
-  if (make_plan(d->outer, d->groups, d->inner, true, true, resident, &a) != FQB200_OK) return 0;
-  if (make_plan(d->outer, d->groups, d->inner, true, false, resident, &b) != FQB200_OK) return 0;
-  if (make_plan(d->outer, d->groups, d->inner, false, false, resident, &c) != FQB200_OK) return 0;
-  uint64_t parts = a.geo.parts;
-  if (b.geo.parts > parts) parts = b.geo.parts;
-  if (c.geo.parts > parts) parts = c.geo.parts;
-  return carve(nullptr, parts * static_cast<uint64_t>(d->groups), static_cast<uint64_t>(d->groups), nullptr);
+  if (d->outer == 0 || d->groups == 0 || d->inner == 0) return 256;
+  const DeviceInfo r = plan_residency();
+  size_t bytes = 0;
+  for (bool can_vec : {false, true}) {  // the aligned plan last: its message stands when both refuse
+    FusedPlan fp;
+    if (plan_fused(d, can_vec, r, &fp) != FQB200_OK) continue;
+    const size_t need = fp.workspace ? fp.workspace : 256;  // RANGE_GIVEN uses none; non-zero = "descriptor accepted"
+    if (need > bytes) bytes = need;
+  }
+  return bytes;
 }
 
 int fqb200_workspace_init(void* workspace, size_t bytes, void* stream) {
@@ -1828,32 +2007,15 @@ int fqb200_plan_info(const fqb200_desc* d, int64_t* out8) {
   int rc = check_desc(d);
   if (rc != FQB200_OK) return rc;
   if (!out8) return fail(FQB200_ERR_INVALID, "null output%s");
-  DeviceInfo* di = nullptr;
-  int resident = kAssumedSms * fqb::kCtasPerSm, resident_cl = kAssumedSms * fqb::kCtasPerSm;
-  if (get_device(&di) == FQB200_OK) {
-    resident = di->resident;
-    resident_cl = di->resident_cl[d->out_hist ? 1 : 0];
-  }
-  Plan pl;
-  if (d->channels_last) {
-    if (!cl_supported(d)) return fail(FQB200_ERR_UNSUPPORTED, "channels_last: per-channel torch / mid-tread leaves, C %% 4 == 0, C <= 2048%s");
-    rc = make_plan_flat(static_cast<uint64_t>(d->outer) * d->groups * d->inner, d->groups, resident_cl, &pl);
-    if (rc != FQB200_OK) return rc;
-    out8[0] = 2; out8[1] = pl.grid; out8[2] = pl.flat.units; out8[3] = pl.flat.unit_stages; out8[4] = pl.flat.stage_v;
-    out8[5] = pl.flat.stride; out8[6] = fqb::kStages; out8[7] = cl_needs_b(d) ? 3 : 2;
-    return FQB200_OK;
-  }
-  if (rows_supported(d, true)) {
-    fqb::RowsGeo rg;
-    rc = make_plan_rows(static_cast<uint64_t>(d->groups), static_cast<uint64_t>(d->inner), d->bias ? -d->bias_period : 0,
-                        di ? di->resident_rows : resident, &pl, &rg);
-    if (rc != FQB200_OK) return rc;
-    out8[0] = 3; out8[1] = pl.grid; out8[2] = pl.flat.units; out8[3] = pl.flat.unit_stages; out8[4] = pl.flat.stage_v;
-    out8[5] = pl.flat.stride; out8[6] = fqb::kStages; out8[7] = 2;
-    return FQB200_OK;
-  }
-  rc = make_plan(d->outer, d->groups, d->inner, true, !(d->bias_corr || d->var_corr), resident, &pl);
+  FusedPlan fp;
+  rc = plan_fused(d, true, plan_residency(), &fp);
   if (rc != FQB200_OK) return rc;
+  const Plan& pl = fp.pl;
+  if (pl.mode == 2 || pl.mode == 3) {  // phases: apply only (RANGE_GIVEN), statistics + apply, + the second statistics pass
+    out8[0] = pl.mode; out8[1] = pl.grid; out8[2] = pl.flat.units; out8[3] = pl.flat.unit_stages; out8[4] = pl.flat.stage_v;
+    out8[5] = pl.flat.stride; out8[6] = fqb::kStages; out8[7] = d->range_mode == FQB200_RANGE_GIVEN ? 1 : 2 + fp.A.need_dev;
+    return FQB200_OK;
+  }
   out8[0] = pl.mode; out8[1] = pl.grid; out8[2] = pl.geo.units; out8[3] = pl.geo.parts; out8[4] = pl.geo.part_v;
   out8[5] = pl.geo.stride; out8[6] = fqb::kRingDepth; out8[7] = pl.geo.red_lanes;
   return FQB200_OK;
@@ -1997,186 +2159,22 @@ int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* worksp
   DeviceInfo* di = nullptr;
   rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
-  Plan pl;
-  if (d->bias && d->bias_period == 0 && d->scope == FQB200_SCOPE_GROUP_MEAN)
-    return fail(FQB200_ERR_UNSUPPORTED, "a per-group bias needs groups = channels (scope GROUP or TENSOR); use bias_period%s");
-  const bool can_vec = aligned16(in) && (d->stats_only || d->pool || aligned16(out));
-  fqb::RowsGeo rows_geo;
-  memset(&rows_geo, 0, sizeof(rows_geo));
-  if (d->channels_last) {
-    if (!can_vec || !cl_supported(d))
-      return fail(FQB200_ERR_UNSUPPORTED, "channels_last: per-channel torch / mid-tread leaves on 16-byte aligned tensors, C %% 4 == 0, C <= 2048%s");
-    rc = make_plan_flat(static_cast<uint64_t>(d->outer) * d->groups * d->inner, d->groups,
-                        d->range_mode == FQB200_RANGE_GIVEN ? di->resident_cl[0] * 2 : di->resident_cl[d->out_hist ? 1 : 0], &pl);
-  } else if (rows_supported(d, can_vec)) {
-    rc = make_plan_rows(static_cast<uint64_t>(d->groups), static_cast<uint64_t>(d->inner), d->bias ? -d->bias_period : 0,
-                        di->resident_rows, &pl, &rows_geo);
-  } else if (d->bias && d->bias_period < 0) {
-    return fail(FQB200_ERR_UNSUPPORTED, "a channel-fastest bias (bias_period < 0) needs the per-sample / per-tensor min-max layout%s");
-  } else {
-    rc = make_plan(d->outer, d->groups, d->inner, can_vec, !(d->bias_corr || d->var_corr), di->resident, &pl);
-  }
+  FusedPlan fp;
+  rc = plan_fused(d, aligned16(in) && (d->stats_only || d->pool || aligned16(out)), *di, &fp);
   if (rc != FQB200_OK) return rc;
-  fqb::FusedArgs A;
-  memset(&A, 0, sizeof(A));
-  // per-unit partial slots; the channels-last kernels combine through the fixed accumulators instead
-  const uint64_t slots = (pl.mode == 2 || pl.mode == 3) ? 0 : static_cast<uint64_t>(pl.geo.parts) * pl.geo.channels;
-  const bool given = d->range_mode == FQB200_RANGE_GIVEN;   // no statistics, no barrier: no workspace
-  if (!given) {
-    const size_t need = carve(nullptr, slots, pl.geo.channels, nullptr);
-    if (!workspace || workspace_bytes < need) return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_workspace_bytes()%s");
+  if (fp.workspace) {
+    if (!workspace || workspace_bytes < fp.workspace) return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_workspace_bytes()%s");
     if (!aligned16(workspace)) return fail(FQB200_ERR_WORKSPACE, "workspace must be 16-byte aligned%s");
-    carve(static_cast<char*>(workspace), slots, pl.geo.channels, &A);
+    carve(static_cast<char*>(workspace), fp.slots, fp.pl.geo.channels, &fp.A);
   }
-  A.geo = pl.geo;
-  A.flat = pl.flat;
-  A.rows = rows_geo;
-  A.in = in;
-  A.out = out;
-  A.scope = d->scope;
-  A.range_mode = d->range_mode;
-  A.leaf = d->leaf;
-  A.num_bits = d->num_bits;
-  A.positive = d->positive;
-  A.solve_f64 = d->solve_f64;
-  A.clip_k = d->clip_k;
-  A.bit_alloc = d->bit_alloc;
-  A.prior = d->bit_alloc_prior;
-  A.ba_round = d->bit_alloc_round;
-  A.ba_target = d->bit_alloc_target;
-  A.mt_target = d->mt_target;
-  A.mt_clip = d->mt_clip;
-  A.bias_corr = d->bias_corr;
-  A.var_corr = d->var_corr;
-  A.stats_only = d->stats_only;
-  A.relu_passthrough = d->relu_passthrough;
-  A.residual = d->residual;
-  A.residual_relu = d->residual_relu;
-  A.residual_stats = d->residual_stats;
-  A.residual_bias = d->residual_bias;
-  if ((d->residual_stats || d->residual_bias) && !d->residual)
-    return fail(FQB200_ERR_INVALID, "residual_stats / residual_bias without a residual%s");
-  if (d->residual_bias && !d->residual_stats)
-    return fail(FQB200_ERR_INVALID, "residual_bias needs residual_stats (a bias on a plain addend can be folded by the caller)%s");
-  if (d->residual && ((!d->channels_last && pl.mode != 3) || d->stats_only || !aligned16(d->residual)))
-    return fail(FQB200_ERR_UNSUPPORTED, "residual: channels-last or per-sample / per-tensor min-max apply launches, 16-byte aligned%s");
-  memset(&A.pool, 0, sizeof(A.pool));
-  A.pool_out = nullptr;
-  if (d->pool) {
-    // channels-last per-channel launches, or the per-sample / per-tensor min-max launches (rows = samples) on channels-last
-    // memory, which know the channel count from their channel-fastest bias
-    const bool rows_cl = pl.mode == 3 && d->bias && d->bias_period < 0;
-    if ((d->pool != 2 && d->pool != 3) || !(d->channels_last || rows_cl) || d->stats_only || d->residual || d->out_hist || !d->pool_out ||
-        !aligned16(d->pool_out))
-      return fail(FQB200_ERR_UNSUPPORTED, "pool: 2 (2x2 stride 2) or 3 (3x3 stride 2 padding 1) on channels-last apply launches without residual / histogram, 16-byte aligned pool_out%s");
-    const int64_t h = d->pool_h, w = d->pool_w;
-    const int64_t hw = rows_cl ? d->inner / -d->bias_period : d->inner;
-    const int64_t images = rows_cl ? d->groups : d->outer;
-    if (h < 2 || w < 2 || w % 2 != 0 || h * w != hw || (d->pool == 3 && h % 2 != 0))
-      return fail(FQB200_ERR_UNSUPPORTED, "pool: pool_h * pool_w must be H * W of the tensor, W even (3x3: H even too)%s");
-    const unsigned cv = pl.flat.cv, stage_v = fqb::kStageVec * fqb::kConsumers;
-    unsigned wt = 0;
-    uint64_t tiles = 0;
-    if (d->pool == 2) {
-      // tile = 2 rows x wt input pixels: two row pieces in the two halves of a stage, (wt / 2) * cv output vectors
-      for (int64_t cand = w; cand >= 2; cand -= 2)
-        if (w % cand == 0 && static_cast<uint64_t>(cand) * cv <= stage_v / 2u && static_cast<uint64_t>(cand / 2) * cv <= pl.flat.stride) {
-          wt = static_cast<unsigned>(cand);
-          break;
-        }
-      if (wt) tiles = static_cast<uint64_t>(images) * static_cast<uint64_t>(h / 2) * static_cast<uint64_t>(w / wt);
-    } else {
-      // tile = 1 output row x wt output pixels: three row pieces of 2 * wt + 1 input pixels in three regions of a stage
-      const int64_t ow = w / 2;
-      for (int64_t cand = ow; cand >= 1; --cand)
-        if (ow % cand == 0 && 3ull * static_cast<uint64_t>(2 * cand + 1) * cv <= stage_v && static_cast<uint64_t>(cand) * cv <= pl.flat.stride) {
-          wt = static_cast<unsigned>(cand);
-          break;
-        }
-      if (wt) tiles = static_cast<uint64_t>(images) * static_cast<uint64_t>(h / 2) * static_cast<uint64_t>(ow / wt);
-    }
-    if (!wt) return fail(FQB200_ERR_UNSUPPORTED, "pool: no tile width fits%s");
-    if (tiles >= 0xfffffff0ull) return fail(FQB200_ERR_UNSUPPORTED, "pool: too many tiles%s");
-    uint64_t unit_tiles = tiles / (kUnitsPerCta * static_cast<uint64_t>(pl.grid));
-    if (unit_tiles < 2) unit_tiles = 2;
-    if (unit_tiles > 64) unit_tiles = 64;
-    A.pool.h = static_cast<unsigned>(h);
-    A.pool.w = static_cast<unsigned>(w);
-    A.pool.wt = wt;
-    A.pool.tiles_per_row = static_cast<unsigned>((d->pool == 2 ? w : w / 2) / wt);
-    A.pool.row_pairs = static_cast<unsigned>(h / 2);
-    A.pool.tiles = static_cast<unsigned>(tiles);
-    A.pool.unit_tiles = static_cast<unsigned>(unit_tiles);
-    A.pool.units = static_cast<unsigned>((tiles + unit_tiles - 1) / unit_tiles);
-    A.pool.ow = static_cast<unsigned>(w / 2);
-    A.pool.kind = static_cast<unsigned>(d->pool);
-    A.pool_out = d->pool_out;
-  }
-  A.out_stats = d->out_stats;
-  A.bias = d->bias;
-  A.hist = d->out_hist;
-  A.hist_bins = d->out_hist ? (d->hist_bins > 0 ? d->hist_bins : 256) : 0;
-  A.hist_offset = d->hist_offset;
-  A.hist_clamped = d->out_hist_clamped;
-  A.dbg = d->debug_stamps;
-  if (d->out_hist && d->leaf != FQB200_LEAF_TORCH && !d->channels_last)
-    return fail(FQB200_ERR_UNSUPPORTED, "out_hist: torch leaf, or the mid-tread leaf on channels-last tensors%s");
-  if (d->out_hist && (A.hist_bins > static_cast<int>(fqb::kHistWords) || (!d->channels_last && A.hist_bins != 256)))
-    return fail(FQB200_ERR_UNSUPPORTED, "hist_bins: 256 (default), up to 8192 on channels-last tensors%s");
-  A.bias_magic = 0;
-  if (given) {
-    A.g_delta = d->given_delta;
-    A.g_offset = d->given_offset;
-    A.g_bits = d->given_bits;
-    A.given_per_group = 1;
-    fqb::fq_cl_given_fused_kernel<<<pl.grid, fqb::kBulkThreads, cl_given_smem(), static_cast<cudaStream_t>(stream)>>>(A);
-    cudaError_t ge = cudaGetLastError();
-    if (ge != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_cl_given_fused_kernel: %s", cudaGetErrorString(ge));
-    return FQB200_OK;
-  }
-  if (pl.mode == 3) {
-    if (d->scope == FQB200_SCOPE_GROUP) A.scope = FQB200_SCOPE_TENSOR;  // one row
-    A.n_per_group = static_cast<double>(d->inner);
-    void* rargs[] = {&A};
-    cudaError_t re = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(fqb::fq_rows_kernel), dim3(pl.grid), dim3(fqb::kBulkThreads),
-                                                 rargs, cl_given_smem(), static_cast<cudaStream_t>(stream));
-    if (re != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_rows_kernel: %s", cudaGetErrorString(re));
-    return FQB200_OK;
-  }
-  if (d->bias && d->bias_period > 0) {
-    // bias indexed by the channel inside the row: needs whole vectors per channel and an exact magic division
-    const uint64_t pv = static_cast<uint64_t>(d->bias_period) / pl.vec;
-    if (pl.mode != 4 || d->leaf != FQB200_LEAF_COMPILED || d->range_mode != FQB200_RANGE_MINMAX || d->bias_corr || d->var_corr ||
-        d->stats_only || d->bias_period % pl.vec != 0 || d->inner % d->bias_period != 0 || pv == 0 ||
-        static_cast<uint64_t>(pl.geo.inner_v) * pv >= (1ull << 40) || pl.geo.inner_v >= (1u << 24))
-      return fail(FQB200_ERR_UNSUPPORTED, "bias_period does not fit this layout%s");
-    A.bias_magic = ((1ull << 40) + pv - 1) / pv;
-  }
-  A.inner = static_cast<unsigned>(d->inner);
-  A.n_per_group = static_cast<double>(d->outer) * static_cast<double>(d->inner);
-  void* args[] = {&A};
+  fp.A.in = in;
+  fp.A.out = out;
+  void* args[] = {&fp.A};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaError_t e;
-  if (pl.mode == 2) {
-    // replicas of the per-channel accumulators: CTA b adds into replica b % rep (same-address atomics serialise in L2)
-    const unsigned r = fqb::kMaxNhwcChannels / static_cast<unsigned>(d->groups);
-    A.nhwc_rep = r < 1u ? 1u : (r > 8u ? 8u : r);
-    A.need_dev = cl_needs_b(d) ? 1 : 0;
-    const bool hist = d->out_hist != nullptr;
-    // (the cooperative launch guarantees the co-residency the grid barriers need)
-    e = cudaLaunchCooperativeKernel(cl_kernel_ptr(d->leaf, A.need_dev != 0, hist), dim3(pl.grid), dim3(fqb::kBulkThreads), args,
-                                    cl_smem(hist), st);
-    if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_cl_kernel: %s", cudaGetErrorString(e));
-    return FQB200_OK;
-  }
-  A.nhwc_rep = 1;
-  const bool alloc = d->bit_alloc && d->num_bits <= 4 && d->scope == FQB200_SCOPE_GROUP && d->leaf != FQB200_LEAF_MIDTREAD;
-  A.need_dev = (d->range_mode != FQB200_RANGE_MINMAX) || alloc || d->var_corr || d->leaf == FQB200_LEAF_MIDTREAD ||
-               (d->stats_only ? 1 : 0);
-  const void* kernel = A.bias_magic ? reinterpret_cast<const void*>(fqb::fq_fused_kernel<4, FQB200_LEAF_COMPILED, false, false, true>)
-                                    : fused_kernel_ptr(pl.mode, d->leaf, A.need_dev != 0, d->bias_corr || d->var_corr);
-  e = cudaLaunchCooperativeKernel(kernel, dim3(pl.grid), dim3(fqb::kThreads), args, dyn_smem(pl.vec), st);
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_fused_kernel: %s", cudaGetErrorString(e));
+  // (the cooperative launch guarantees the co-residency the grid barriers need)
+  const cudaError_t e = fp.coop ? cudaLaunchCooperativeKernel(fp.kernel, dim3(fp.pl.grid), dim3(fp.block), args, fp.smem, st)
+                                : cudaLaunchKernel(fp.kernel, dim3(fp.pl.grid), dim3(fp.block), args, fp.smem, st);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, fp.coop ? "cooperative launch %s: %s" : "launch %s: %s", fp.name, cudaGetErrorString(e));
   return FQB200_OK;
 }
 

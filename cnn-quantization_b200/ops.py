@@ -387,7 +387,7 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
         stream = _stream_handle(dev)
         need = lib.fqb200_workspace_bytes(ctypes.byref(d))
         if need == 0:
-            L.check(L.ERR_INVALID if not lib.fqb200_last_error() else L.ERR_INVALID)
+            L.check(L.ERR_INVALID)
         ws = _workspace(dev, stream, need)
         two_pass = (range_mode != L.RANGE_MINMAX or leaf == L.LEAF_MIDTREAD or var_corr or stats_only or
                     (bit_alloc and num_bits <= 4 and scope == L.SCOPE_GROUP))

@@ -167,9 +167,11 @@ const char* fqb200_last_error(void);
 /* number of CTAs the fused kernel keeps resident on the current device (132 SMs x 2 on an H100) */
 int fqb200_resident_ctas(void);
 
-/* What a launch of `d` would look like on the current device (introspection for tools and tests), 8 values:
+/* The launch fqb200_fused makes for `d` with 16-byte-aligned tensors on the current device (an H100 when there is none),
+ * or the code and message with which it refuses `d` (introspection for tools and tests), 8 values:
  * channels_last, and the per-sample / per-tensor min-max layouts ({3, ...}) on the bulk-copy engine:
- *                {2, grid, units, stages per unit, vectors per stage, consumer stride, ring stages, phases};
+ *                {2, grid, units, stages per unit, vectors per stage, consumer stride, ring stages, phases}
+ *                (phases: 1 for FQB200_RANGE_GIVEN, which only applies);
  * otherwise:     {access mode 4|1|8, grid, units, parts per group, vectors per part, stride, ring depth, leader lanes}. */
 int fqb200_plan_info(const fqb200_desc* d, int64_t* out8);
 /* Self-test hook: fast[i] = the kernels' 3-instruction exact division a[i] / b[i], ieee[i] = IEEE a[i] / b[i]
