@@ -19,7 +19,8 @@ STAT_COLUMNS = ("min", "max", "mean", "b", "std", "delta", "offset", "bits", "sc
 # every symbol include/fqb200.h declares (tests check the export table against this)
 SYMBOLS = ("fqb200_abi_version", "fqb200_last_error", "fqb200_resident_ctas", "fqb200_plan_info",
            "fqb200_selftest_division", "fqb200_workspace_bytes", "fqb200_workspace_init", "fqb200_float2gemmlowp",
-           "fqb200_quantize1", "fqb200_quantize1_bca", "fqb200_fused", "fqb200_add_relu", "fqb200_maxpool2d_nhwc",
+           "fqb200_quantize1", "fqb200_quantize1_bca", "fqb200_fused", "fqb200_fused_into", "fqb200_add_relu",
+           "fqb200_maxpool2d_nhwc", "fqb200_maxpool2d_nhwc_into",
            "fqb200_kld_threshold", "fqb200_kld_workspace_bytes", "fqb200_sample_sumsq",
            "fqb200_sample_sumsq_workspace_bytes", "fqb200_clip_error", "fqb200_clip_error_workspace_bytes",
            "fqb200_kmeans1d", "fqb200_kmeans1d_workspace_bytes")
@@ -86,10 +87,14 @@ def load():
     lib.fqb200_quantize1.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, vp, i32, i32, vp, i32, vp]
     lib.fqb200_fused.restype = i32
     lib.fqb200_fused.argtypes = [ctypes.POINTER(Desc), vp, vp, vp, ctypes.c_size_t, vp]
+    lib.fqb200_fused_into.restype = i32
+    lib.fqb200_fused_into.argtypes = [ctypes.POINTER(Desc), vp, vp, i64, vp, ctypes.c_size_t, vp]
     lib.fqb200_quantize1_bca.restype = i32
     lib.fqb200_quantize1_bca.argtypes = [vp, vp, i64, i64, i64, vp, vp, vp, i32, i32, vp, i32, vp, vp, ctypes.c_size_t, vp]
     lib.fqb200_maxpool2d_nhwc.restype = i32
     lib.fqb200_maxpool2d_nhwc.argtypes = [vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, i32, vp]
+    lib.fqb200_maxpool2d_nhwc_into.restype = i32
+    lib.fqb200_maxpool2d_nhwc_into.argtypes = [vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, i32, i64, vp]
     lib.fqb200_add_relu.restype = i32
     lib.fqb200_add_relu.argtypes = [vp, vp, vp, i64, vp]
     lib.fqb200_selftest_division.restype = i32

@@ -296,7 +296,9 @@ struct ClApply {
         if (A.residual_relu) y[i] = y[i] < 0.f ? 0.f : y[i];
       }
     }
-    st_tensor(reinterpret_cast<float4*>(A.out) + off, make_float4(y[0], y[1], y[2], y[3]));
+    // a channel slice of a wider tensor (out_pad_v): `off` counts cv vectors per pixel, the output out_pad_v more
+    const unsigned o = A.out_pad_v ? off + (off / A.flat.cv) * A.out_pad_v : off;
+    st_tensor(reinterpret_cast<float4*>(A.out) + o, make_float4(y[0], y[1], y[2], y[3]));
     if (HIST) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) count(i, gq[i]);

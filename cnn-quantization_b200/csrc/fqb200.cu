@@ -54,6 +54,8 @@ struct FusedArgs {
   RowsGeo rows;        // ... row structure of the per-sample min-max kernel
   const float* in;
   float* out;
+  unsigned out_pad_v;     // channels-last apply: a channel slice of a wider tensor is written, (pixel pitch - C) / 4 vectors
+                          // skipped after every pixel (fqb200_fused_into); 0: `out` is dense like `in`
   const float* residual;  // channels-last kernel: optional tensor added to the quantized values (fqb200_desc.residual)
   int residual_relu;      // ... followed by max(., 0)
   PoolGeo pool;           // channels-last kernel: 2x2 / stride-2 max pooling inside the apply phase (pool.tiles != 0) ...
@@ -1199,6 +1201,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 struct PoolArgs {
   const float* in;
   float* out;
+  unsigned long long out_pv;  // output pixel pitch in vectors (cv: dense)
   unsigned n, h, w, cv, oh, ow;
   int kh, kw, sh, sw, ph, pw;
   unsigned long long total;  // output vectors
@@ -1210,7 +1213,8 @@ __global__ void __launch_bounds__(256, 4) fq_maxpool_nhwc_kernel(const __grid_co
   auto upd = [](float& m, float v) { m = (v > m || v != v) ? v : m; };
   for (unsigned long long i = static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < P.total; i += stride) {
     const unsigned c = static_cast<unsigned>(i % P.cv);
-    unsigned long long r = i / P.cv;
+    const unsigned long long pixel = i / P.cv;
+    unsigned long long r = pixel;
     const unsigned ow = static_cast<unsigned>(r % P.ow);
     r /= P.ow;
     const unsigned oh = static_cast<unsigned>(r % P.oh);
@@ -1232,7 +1236,7 @@ __global__ void __launch_bounds__(256, 4) fq_maxpool_nhwc_kernel(const __grid_co
         upd(m.w, v.w);
       }
     }
-    __stcs(out + i, m);
+    __stcs(out + pixel * P.out_pv + c, m);
   }
 }
 
@@ -1789,6 +1793,22 @@ unsigned pool_tile_width(int kind, int64_t w, const fqb::FlatGeo& f) {
   return 0;
 }
 
+// What a pitched `out` (fqb200_fused_into, `pitch` floats between two pixels) needs beyond the descriptor's own route: the
+// apply phase of a channels-last launch without pooling / residual is the only store that can skip the other channels of a
+// pixel; a 16-byte aligned `out` (`can_vec`); and 32-bit vector offsets.  No CUDA calls: fqb200_fused_into checks it before
+// any device call, plan_fused again for the plan it makes.
+int pitch_rules(const fqb200_desc* d, bool can_vec, int64_t pitch) {
+  if (!d->channels_last || d->stats_only || d->pool || d->residual)
+    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride: channels-last apply launches without pooling / residual only%s");
+  if (pitch < d->groups || pitch % 4 != 0)
+    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride must be >= C and a multiple of 4%s");
+  if (!can_vec) return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride needs 16-byte aligned tensors%s");
+  const uint64_t pixels = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->inner);
+  if (pixels * static_cast<uint64_t>(pitch) / 4 >= (1ull << 32))
+    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride: outputs of 2^32 vectors and more are not supported%s");
+  return FQB200_OK;
+}
+
 // One fqb200_fused launch: route, geometry, kernel and its arguments, all but in / out and the workspace pointers.
 struct FusedPlan {
   Plan pl;                    // mode 2: channels-last flat stream, 3: rows, 4 / 1 / 8: fq_fused_kernel
@@ -1803,8 +1823,9 @@ struct FusedPlan {
 };
 
 // The single place where a fused descriptor's route is decided and refused.  `d` passed check_desc; `can_vec`: in / out
-// are 16-byte aligned; `r` holds the resident-CTA counts the grids are sized for.  No CUDA calls.
-int plan_fused(const fqb200_desc* d, bool can_vec, const DeviceInfo& r, FusedPlan* fp) {
+// are 16-byte aligned; `out_pitch`: floats between two pixels of `out` when it is a channel slice of a wider channels-last
+// tensor (fqb200_fused_into), 0 when `out` is dense; `r` holds the resident-CTA counts the grids are sized for.  No CUDA calls.
+int plan_fused(const fqb200_desc* d, bool can_vec, int64_t out_pitch, const DeviceInfo& r, FusedPlan* fp) {
   memset(fp, 0, sizeof(*fp));
   Plan& pl = fp->pl;
   fqb::FusedArgs& A = fp->A;
@@ -1829,6 +1850,11 @@ int plan_fused(const fqb200_desc* d, bool can_vec, const DeviceInfo& r, FusedPla
     rc = make_plan(d->outer, d->groups, d->inner, can_vec, !(d->bias_corr || d->var_corr), r.resident, &pl);
   }
   if (rc != FQB200_OK) return rc;
+  if (out_pitch) {
+    rc = pitch_rules(d, can_vec, out_pitch);
+    if (rc != FQB200_OK) return rc;
+    A.out_pad_v = static_cast<unsigned>((out_pitch - d->groups) / 4);
+  }
   if ((d->residual_stats || d->residual_bias) && !d->residual)
     return fail(FQB200_ERR_INVALID, "residual_stats / residual_bias without a residual%s");
   if (d->residual_bias && !d->residual_stats)
@@ -1987,7 +2013,7 @@ size_t fqb200_workspace_bytes(const fqb200_desc* d) {
   size_t bytes = 0;
   for (bool can_vec : {false, true}) {  // the aligned plan last: its message stands when both refuse
     FusedPlan fp;
-    if (plan_fused(d, can_vec, r, &fp) != FQB200_OK) continue;
+    if (plan_fused(d, can_vec, 0, r, &fp) != FQB200_OK) continue;
     const size_t need = fp.workspace ? fp.workspace : 256;  // RANGE_GIVEN uses none; non-zero = "descriptor accepted"
     if (need > bytes) bytes = need;
   }
@@ -2008,7 +2034,7 @@ int fqb200_plan_info(const fqb200_desc* d, int64_t* out8) {
   if (rc != FQB200_OK) return rc;
   if (!out8) return fail(FQB200_ERR_INVALID, "null output%s");
   FusedPlan fp;
-  rc = plan_fused(d, true, plan_residency(), &fp);
+  rc = plan_fused(d, true, 0, plan_residency(), &fp);
   if (rc != FQB200_OK) return rc;
   const Plan& pl = fp.pl;
   if (pl.mode == 2 || pl.mode == 3) {  // phases: apply only (RANGE_GIVEN), statistics + apply, + the second statistics pass
@@ -2149,6 +2175,11 @@ int fqb200_quantize1(const float* in, float* out, float* grid, int64_t outer, in
 
 int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* workspace, size_t workspace_bytes,
                  void* stream) {
+  return fqb200_fused_into(d, in, out, 0, workspace, workspace_bytes, stream);
+}
+
+int fqb200_fused_into(const fqb200_desc* d, const float* in, float* out, int64_t out_pixel_stride, void* workspace,
+                      size_t workspace_bytes, void* stream) {
   g_err[0] = 0;
   int rc = check_desc(d);
   if (rc != FQB200_OK) return rc;
@@ -2156,11 +2187,23 @@ int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* worksp
   if (!in) return fail(FQB200_ERR_INVALID, "null input%s");
   if (!out && !d->stats_only && !d->pool) return fail(FQB200_ERR_INVALID, "null output%s");
   if (d->stats_only && !d->out_stats) return fail(FQB200_ERR_INVALID, "stats_only needs out_stats%s");
+  const bool can_vec = aligned16(in) && (d->stats_only || d->pool || aligned16(out));
+  if (out_pixel_stride != 0) {   // 0: fqb200_fused, a dense `out`
+    if (out_pixel_stride < 0) return fail(FQB200_ERR_INVALID, "negative out_pixel_stride%s");
+    rc = pitch_rules(d, can_vec, out_pixel_stride);
+    if (rc != FQB200_OK) return rc;
+    const uint64_t pixels = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->inner);
+    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), i1 = i0 + pixels * d->groups * sizeof(float);
+    const uintptr_t o0 = reinterpret_cast<uintptr_t>(out),
+                    o1 = o0 + ((pixels - 1) * out_pixel_stride + d->groups) * sizeof(float);
+    if (out_pixel_stride != d->groups && o0 < i1 && i0 < o1)   // (the dense case may work in place)
+      return fail(FQB200_ERR_INVALID, "out_pixel_stride: out overlaps in%s");
+  }
   DeviceInfo* di = nullptr;
   rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   FusedPlan fp;
-  rc = plan_fused(d, aligned16(in) && (d->stats_only || d->pool || aligned16(out)), *di, &fp);
+  rc = plan_fused(d, can_vec, out_pixel_stride == d->groups ? 0 : out_pixel_stride, *di, &fp);   // pitch C: dense
   if (rc != FQB200_OK) return rc;
   if (fp.workspace) {
     if (!workspace || workspace_bytes < fp.workspace) return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_workspace_bytes()%s");
@@ -2223,19 +2266,30 @@ int fqb200_quantize1_bca(const float* in, float* out, int64_t outer, int64_t gro
 
 int fqb200_maxpool2d_nhwc(const float* in, float* out, int64_t n, int64_t h, int64_t w, int64_t c, int kh, int kw, int sh, int sw,
                           int ph, int pw, void* stream) {
+  return fqb200_maxpool2d_nhwc_into(in, out, n, h, w, c, kh, kw, sh, sw, ph, pw, c, stream);
+}
+
+int fqb200_maxpool2d_nhwc_into(const float* in, float* out, int64_t n, int64_t h, int64_t w, int64_t c, int kh, int kw, int sh,
+                               int sw, int ph, int pw, int64_t out_pixel_stride, void* stream) {
   g_err[0] = 0;
   if (n < 0 || h <= 0 || w <= 0 || c <= 0 || kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || ph < 0 || pw < 0 || 2 * ph > kh || 2 * pw > kw)
     return fail(FQB200_ERR_INVALID, "bad pooling geometry%s");
   if (n == 0) return FQB200_OK;
   if (!in || !out) return fail(FQB200_ERR_INVALID, "null tensor pointer%s");
   if (c % 4 != 0 || !aligned16(in) || !aligned16(out)) return fail(FQB200_ERR_UNSUPPORTED, "channels-last pooling needs C %% 4 == 0 and 16-byte aligned tensors%s");
+  if (out_pixel_stride < c || out_pixel_stride % 4 != 0)
+    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride must be >= C and a multiple of 4%s");
   const int64_t oh = (h + 2 * ph - kh) / sh + 1, ow = (w + 2 * pw - kw) / sw + 1;
   if (oh <= 0 || ow <= 0 || h >= (1ll << 31) || w >= (1ll << 31) || n >= (1ll << 31)) return fail(FQB200_ERR_INVALID, "bad pooling geometry%s");
+  const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), i1 = i0 + static_cast<uint64_t>(n * h * w * c) * sizeof(float);
+  const uintptr_t o0 = reinterpret_cast<uintptr_t>(out),
+                  o1 = o0 + static_cast<uint64_t>((n * oh * ow - 1) * out_pixel_stride + c) * sizeof(float);
+  if (o0 < i1 && i0 < o1) return fail(FQB200_ERR_INVALID, "out overlaps in%s");
   DeviceInfo* di = nullptr;
   int rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   fqb::PoolArgs P;
-  P.in = in; P.out = out;
+  P.in = in; P.out = out; P.out_pv = static_cast<unsigned long long>(out_pixel_stride / 4);
   P.n = static_cast<unsigned>(n); P.h = static_cast<unsigned>(h); P.w = static_cast<unsigned>(w); P.cv = static_cast<unsigned>(c / 4);
   P.oh = static_cast<unsigned>(oh); P.ow = static_cast<unsigned>(ow);
   P.kh = kh; P.kw = kw; P.sh = sh; P.sw = sw; P.ph = ph; P.pw = pw;

@@ -106,13 +106,13 @@ class IntQuantizer(object):
         self.export_stats = False
         self.last_stats = None
         # per-call inputs of ``__call__``'s extensions (reset when the call returns)
-        self._relu_follows, self._bca, self._residual, self._defer, self._pool = False, None, None, False, None
+        self._relu_follows, self._bca, self._residual, self._defer, self._pool, self._into = False, None, None, False, None, None
 
     # ------------------------------------------------------------------------------------------
     # dispatch (int_quantizer.py:92-122)
     # ------------------------------------------------------------------------------------------
     def __call__(self, tensor, id, tag="", stat_id=None, override_att=None, weight_correction=None, bias=None,
-                 relu_follows=False, bias_correct=None, residual=None, defer=False, pool=None):
+                 relu_follows=False, bias_correct=None, residual=None, defer=False, pool=None, out=None):
         """Extensions used by this package's manager (all default to the reference behaviour):
         ``bias_correct`` (None = off, else the "ReLU follows" flag of the call site): the activation bias correction of
         Conv2dWithId.forward (`-bca`, inference_quantization_manager.py:180-196) is applied by the quantizer itself - inside
@@ -136,7 +136,10 @@ class IntQuantizer(object):
         ``weight_correction=(bias_corr, var_corr)``: the per-output-channel mean / variance correction of
         inference_quantization_manager.py:374-391 is applied inside the same launch that quantizes the weight;
         ``bias``: a per-channel vector added to the tensor before anything else inside the kernel (the folded-BN
-        convolution bias, so the convolution itself can run bias-free and a whole pass over the activation is saved)."""
+        convolution bias, so the convolution itself can run bias-free and a whole pass over the activation is saved);
+        ``out``: a channel slice of a wider channels-last tensor (a branch's part of an Inception block's concatenation);
+        where the channels-last apply launch can write it (``ops.slice_eligible``) the result is written there and that
+        slice comes back; otherwise the operand is ignored and the caller copies the result itself."""
         if override_att is not None:
             orig_att = getattr(self, override_att[0])
             setattr(self, override_att[0], override_att[1])
@@ -145,6 +148,7 @@ class IntQuantizer(object):
         self._residual = residual
         self._defer = bool(defer)
         self._pool = tuple(pool) if pool is not None else None
+        self._into = out
         try:
             self._unsupported(stat_id)
             if bias is not None and not self._bias_fusable(tensor):
@@ -176,7 +180,7 @@ class IntQuantizer(object):
         finally:
             if override_att is not None:
                 setattr(self, override_att[0], orig_att)
-            self._relu_follows, self._bca, self._residual, self._defer, self._pool = False, None, None, False, None
+            self._relu_follows, self._bca, self._residual, self._defer, self._pool, self._into = False, None, None, False, None, None
         return res
 
     def __repr__(self):
@@ -267,7 +271,7 @@ class IntQuantizer(object):
         """Mode A launch; with ``bias_correct`` set the activation bias correction rides along."""
         if self._bca is None or tensor.dim() != 4:
             # per-channel parameters of a channels-last tensor that the descriptor entry point takes as it is
-            if ((self._defer or self._residual is not None or self._pool is not None) and layout is not None
+            if ((self._defer or self._residual is not None or self._pool is not None or self._into is not None) and layout is not None
                     and torch.is_tensor(delta) and delta.numel() == layout[1] and not self.measure_entropy
                     and ops.cl_eligible(tensor, layout)):
                 if self._defer:
@@ -345,6 +349,8 @@ class IntQuantizer(object):
                 res._fq_pooled = pool[0]   # 2 / 3: which pooling the launch has done
                 return res
         rkw = self._residual_kw(tensor, channels_last, rows=rows, bias=kw.get("bias"))
+        if not rkw and self._into is not None and ops.slice_eligible(tensor, self._into, channels_last):
+            kw["out"] = self._into
         res = self._fused(tensor, layout, channels_last=channels_last, **kw, **rkw)
         if rkw:
             res._fq_residual_fused = True

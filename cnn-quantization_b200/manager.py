@@ -237,6 +237,95 @@ def _residual_block_forward(block, bottleneck, manager):
     return forward
 
 
+def _basic_conv_forward(block):
+    """forward of a torchvision Inception ``BasicConv2d`` (conv -> bn -> ``F.relu(x, inplace=True)``) that returns tensors
+    tagged non-negative by the quantizer untouched, as the hooked nn.ReLU modules do (_relu_forward_skipping): the functional
+    ReLU is no module, so nothing else can skip it."""
+    import torch.nn.functional as F
+
+    def forward(x):
+        x = block.bn(block.conv(x))
+        if getattr(x, "_fq_nonneg", None) == x._version:
+            return x
+        return F.relu(x, inplace=True)
+
+    return forward
+
+
+# The branches of torchvision's Inception blocks (torchvision/models/inception.py), in the order their forward runs them:
+# BasicConv2d names applied one after the other; a tuple is InceptionE's pair of convolutions on the same input whose
+# outputs are concatenated; "avg" / "max" are the functional F.avg_pool2d(x, 3, 1, 1) / F.max_pool2d(x, 3, 2).
+_INCEPTION_BRANCHES = {
+    "InceptionA": (("branch1x1",), ("branch5x5_1", "branch5x5_2"), ("branch3x3dbl_1", "branch3x3dbl_2", "branch3x3dbl_3"),
+                   ("avg", "branch_pool")),
+    "InceptionB": (("branch3x3",), ("branch3x3dbl_1", "branch3x3dbl_2", "branch3x3dbl_3"), ("max",)),
+    "InceptionC": (("branch1x1",), ("branch7x7_1", "branch7x7_2", "branch7x7_3"),
+                   ("branch7x7dbl_1", "branch7x7dbl_2", "branch7x7dbl_3", "branch7x7dbl_4", "branch7x7dbl_5"), ("avg", "branch_pool")),
+    "InceptionD": (("branch3x3_1", "branch3x3_2"), ("branch7x7x3_1", "branch7x7x3_2", "branch7x7x3_3", "branch7x7x3_4"), ("max",)),
+    "InceptionE": (("branch1x1",), ("branch3x3_1", ("branch3x3_2a", "branch3x3_2b")),
+                   ("branch3x3dbl_1", "branch3x3dbl_2", ("branch3x3dbl_3a", "branch3x3dbl_3b")), ("avg", "branch_pool")),
+}
+
+
+def _inception_block_forward(block, manager):
+    """forward of a torchvision InceptionA..E whose branches write their outputs straight into the block's channels-last
+    output instead of ``torch.cat``-ing them afterwards (a re-read and re-write of every branch output): the output is
+    allocated once, each branch's last convolution gets its channel slice as ``_fq_out`` (the conv hook hands it to the
+    quantization launch, which writes it in place), and the max-pool branch pools into its slice.  Same call sites in the
+    same order, bit-identical results.  Anything but a channels-last fp32 CUDA input runs the block's own forward."""
+    import torch.nn.functional as F
+    from . import ops
+
+    orig = type(block).forward
+    branches = _INCEPTION_BRANCHES[type(block).__name__]
+
+    def width(step, x):
+        if step == "max":
+            return x.shape[1]
+        names = step if isinstance(step, tuple) else (step,)
+        return sum(getattr(block, k).conv.out_channels for k in names)
+
+    def into(name, x, sl):
+        basic = getattr(block, name)
+        basic.conv._fq_out = sl
+        try:
+            y = basic(x)
+        finally:
+            basic.conv.__dict__.pop("_fq_out", None)
+        if y.data_ptr() != sl.data_ptr() or y.stride() != sl.stride():
+            sl.copy_(y)   # the launch could not write the slice
+
+    def forward(x):
+        widths = [width(b[-1], x) for b in branches]
+        if not (manager.fuse_inception_concat and manager.enabled and x.is_cuda and x.dtype == torch.float32 and ops.nhwc(x)
+                and not x.requires_grad and all(ops.cl_channels_ok(c) for c in widths) and x.shape[1] % 4 == 0):
+            return orig(block, x)
+        n, _, h, w = x.shape
+        oh, ow = ((h - 3) // 2 + 1, (w - 3) // 2 + 1) if branches[-1] == ("max",) else (h, w)
+        out = torch.empty((n, sum(widths), oh, ow), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        c0 = 0
+        for steps, c in zip(branches, widths):
+            sl = out[:, c0:c0 + c]
+            y = x
+            for step in steps[:-1]:
+                y = F.avg_pool2d(y, kernel_size=3, stride=1, padding=1) if step == "avg" else getattr(block, step)(y)
+            last = steps[-1]
+            if last == "max":
+                ops.maxpool2d_cl(y, 3, 2, 0, out=sl)
+            elif isinstance(last, tuple):   # InceptionE: the inner concatenation's parts go to their final places
+                k0 = 0
+                for name in last:
+                    k = getattr(block, name).conv.out_channels
+                    into(name, y, sl[:, k0:k0 + k])
+                    k0 += k
+            else:
+                into(last, y, sl)
+            c0 += c
+        return out
+
+    return forward
+
+
 class QuantizationManagerInference(object):
     """``with QuantizationManagerInference(args, qparams) as qm: model = build(); qm.attach(model); qm.quantize_model(model)``.
 
@@ -279,6 +368,9 @@ class QuantizationManagerInference(object):
         self.fuse_pool_into_quant = self._native
         # channels-last max pooling in front of the `activation_pooling` call site runs on this package's kernel
         self.fast_maxpool = self._native
+        # the branches of a torchvision Inception block write their (quantized) outputs into the block's output directly,
+        # without the closing torch.cat (not with `-bca`, whose launch writes no channel slice)
+        self.fuse_inception_concat = self._native and not self.bcorr_act
         self.inplace_activations = self._native
         # `-ms` (inference_quantization_manager.py:320-323): the per-sample squared norm of the tensor every conv / linear /
         # non-absorbed BN call site hands on.  Three launches never write that tensor - the block epilogue writes
@@ -292,6 +384,7 @@ class QuantizationManagerInference(object):
             from .statistics import MeasureStatistics
             self.measure_stats = MeasureStatistics(args.arch, getattr(args, "stats_base_dir", None))
             self.fuse_residual_into_quant = self.defer_shortcut = self.fuse_pool_into_quant = False
+            self.fuse_inception_concat = False   # the hooked output is the tensor -ms measures; keep torch.cat's
         # `collect_err`: the collect hooks hand each tensor's use-mode quantizer settings to save_tensor_stats, which fills
         # the mse_* / cos_* columns `-c mix` chooses by
         self.collect_err = bool(getattr(args, "collect_err", False))
@@ -453,6 +546,18 @@ class QuantizationManagerInference(object):
                 if type(m) in (BasicBlock, Bottleneck) and type(getattr(m, "relu", None)) is nn.ReLU:
                     m.forward = _residual_block_forward(m, type(m) is Bottleneck, self)
                     self._patched.append(m)
+        if self.enabled and self.stats_mode != "collect" and self.measure_stats is None:
+            try:
+                from torchvision.models import inception as tv_inception
+            except ImportError:  # pragma: no cover
+                tv_inception = None
+            for m in model.modules() if tv_inception is not None else ():
+                if type(m) is tv_inception.BasicConv2d and self.skip_redundant_relu:
+                    m.forward = _basic_conv_forward(m)
+                    self._patched.append(m)
+                elif self.fuse_inception_concat and type(m).__name__ in _INCEPTION_BRANCHES and type(m) is getattr(tv_inception, type(m).__name__):
+                    m.forward = _inception_block_forward(m, self)
+                    self._patched.append(m)
         if self.fuse_pool_into_quant and self.fast_maxpool and self.skip_redundant_relu and self.enabled and self.stats_mode in ("no", "use"):
             two = lambda v: (v, v) if isinstance(v, int) else tuple(v)
 
@@ -469,8 +574,9 @@ class QuantizationManagerInference(object):
                     self._pool_marked.append(conv)
 
             for seq in model.modules():
-                if isinstance(seq, nn.Sequential):   # VGG: Conv2d, [ReLU,] MaxPool2d
-                    kids = list(seq.children())
+                if isinstance(seq, nn.Sequential):   # VGG: Conv2d, [BatchNorm2d (folded away),] [ReLU,] MaxPool2d
+                    kids = [k for k in seq.children()
+                            if not (self.bn_folding and type(k) is nn.BatchNorm2d and hasattr(k, "absorbed"))]
                     for i, conv in enumerate(kids):
                         nxt = kids[i + 1:i + 3]
                         if len(nxt) >= 1 and type(nxt[0]) is nn.MaxPool2d:
@@ -592,6 +698,9 @@ class QuantizationManagerInference(object):
             # aborted forward is overwritten here
             pm[0]._fq_pending = bool(getattr(res, "_fq_pooled", False))
             return res
+        into = m.__dict__.get("_fq_out")
+        if into is not None and self._native and tag == "activation":
+            extra["out"] = into   # an Inception branch: its part of the block's output, written in place where the launch can
         if m.__dict__.get("_fq_defer") and self._native and tag == "activation":
             res = self.quantize_instant(out, activation_id, tag, stat_id=self._stat_id(activation_id), half_range=half_range,
                                         verbose=self.verbose, defer=True, **extra)

@@ -107,6 +107,34 @@ def cl_eligible(x, layout=None):
     return cl_channels_ok(c) and x.data_ptr() % 16 == 0
 
 
+def slice_pitch(out):
+    """Floats between two pixels of ``out`` when it is an [N, C, H, W] channel slice of a wider channels-last tensor (channel
+    stride 1, rows and images packed at that pixel pitch), else 0."""
+    if out.dim() != 4 or out.stride(1) != 1:
+        return 0
+    p = out.stride(3)
+    return p if out.stride(2) == out.shape[3] * p and out.stride(0) == out.shape[2] * out.shape[3] * p else 0
+
+
+def _overlaps(x, out, pitch):
+    pixels = out.numel() // max(out.shape[1], 1)
+    x0, o0 = x.data_ptr(), out.data_ptr()
+    return o0 < x0 + 4 * x.numel() and x0 < o0 + 4 * ((pixels - 1) * pitch + out.shape[1])
+
+
+def slice_eligible(x, out, channels_last=True, stats_only=False, pool=None, residual=None):
+    """True when a launch of ``fused`` on ``x`` writes ``out``, a channel slice of a wider channels-last tensor
+    (``slice_pitch``), in place (C ABI fqb200_fused_into; the library applies the same rules): a channels-last apply launch
+    without pooling or residual on a ``cl_eligible`` x, the pixel pitch >= C and a multiple of 4, ``out`` 16-byte aligned,
+    not overlapping x."""
+    if (not channels_last or stats_only or pool is not None or residual is not None or not cl_eligible(x)
+            or tuple(out.shape) != tuple(x.shape)):
+        return False
+    p = slice_pitch(out)
+    return (p >= x.shape[1] and p % 4 == 0 and out.data_ptr() % 16 == 0 and not _overlaps(x, out, p)
+            and (out.numel() // x.shape[1]) * p // 4 < 2 ** 32)
+
+
 def rows_eligible(x, other=None):
     """True when the per-sample / per-tensor min-max kernel takes the 4-D ``x`` (and ``other``, an operand read alongside)
     as it is: dense, N <= 4096 samples of a multiple of 4 elements, 16-byte aligned (rows_supported in fqb200.cu)."""
@@ -271,7 +299,8 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     """C ABI fqb200_fused: statistics -> parameters -> quantize/dequantize in one launch.
 
     Returns ``out`` (or ``(out, stats)`` with ``want_stats``; ``stats`` alone with ``stats_only``), where
-    ``stats`` is a [groups, 12] tensor with columns ``_lib.STAT_COLUMNS``."""
+    ``stats`` is a [groups, 12] tensor with columns ``_lib.STAT_COLUMNS``.  A channels-last launch writes an ``out`` that is
+    a channel slice of a wider channels-last tensor directly (``slice_eligible``; profile mode suffix "i")."""
     _require_cuda_f32(x, "tensor")
     lib = L.load()
     is_cl = x.dim() == 4 and x.is_contiguous(memory_format=torch.channels_last)
@@ -382,7 +411,14 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     if x.numel() == 0:
         res = pooled if pooled is not None else x.clone()
         return stats if stats_only else ((res, stats) if want_stats else res)
-    kout, uout = (None, None) if (stats_only or pooled is not None) else _resolve_out(x, out)
+    pitch = 0
+    if stats_only or pooled is not None:
+        kout, uout = None, None
+    elif out is not None and out.stride() != x.stride() and slice_eligible(x, out, channels_last, residual=residual):
+        _require_cuda_f32(out, "out")
+        kout, uout, pitch = out, None, slice_pitch(out)
+    else:
+        kout, uout = _resolve_out(x, out)
     with torch.cuda.device(dev):
         stream = _stream_handle(dev)
         need = lib.fqb200_workspace_bytes(ctypes.byref(d))
@@ -399,9 +435,11 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
             mode, bpe = mode + "r", bpe + 4
         if pooled is not None:     # the apply phase reads x (3x3: rows twice, the second time mostly out of L2) and writes a quarter
             mode, bpe = mode + "p", bpe - 3
+        if pitch:                  # written into a channel slice of a wider tensor
+            mode += "i"
         with _Timed(mode, x.numel(), bpe, "%dx%dx%d" % (outer, groups, inner)):
-            L.check(lib.fqb200_fused(ctypes.byref(d), x.data_ptr(), kout.data_ptr() if kout is not None else None,
-                                     ws.data_ptr(), ws.numel(), stream))
+            L.check(lib.fqb200_fused_into(ctypes.byref(d), x.data_ptr(), kout.data_ptr() if kout is not None else None,
+                                          pitch, ws.data_ptr(), ws.numel(), stream))
     if stats_only:
         return stats
     if pooled is not None:
@@ -611,9 +649,10 @@ def add_relu_(a, b):
     return a
 
 
-def maxpool2d_cl(x, kernel_size, stride, padding):
+def maxpool2d_cl(x, kernel_size, stride, padding, out=None):
     """``F.max_pool2d(x, kernel_size, stride, padding)`` for a channels-last fp32 activation with C % 4 == 0 (C ABI
-    fqb200_maxpool2d_nhwc); the result is channels-last as well.  Bit-identical to torch."""
+    fqb200_maxpool2d_nhwc_into); the result is channels-last as well.  Bit-identical to torch.  ``out``: where to write it,
+    directly when it is a channel slice of a wider channels-last tensor (profile mode "Pi"), else through a copy."""
     _require_cuda_f32(x, "input")
     if x.dim() != 4 or not x.is_contiguous(memory_format=torch.channels_last) or x.shape[1] % 4 != 0:
         raise ValueError("maxpool2d_cl needs a channels-last [N, C, H, W] tensor with C % 4 == 0")
@@ -622,11 +661,18 @@ def maxpool2d_cl(x, kernel_size, stride, padding):
     ph, pw = (padding, padding) if isinstance(padding, int) else padding
     n, c, h, w = x.shape
     oh, ow = (h + 2 * ph - kh) // sh + 1, (w + 2 * pw - kw) // sw + 1
-    out = torch.empty((n, c, oh, ow), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
-    with torch.cuda.device(x.device), _Timed("P", out.numel(), 4 + 4 * sh * sw):
-        L.check(L.load().fqb200_maxpool2d_nhwc(x.data_ptr(), out.data_ptr(), n, h, w, c, kh, kw, sh, sw, ph, pw,
-                                               _stream_handle(x.device)))
-    return out
+    user = out
+    if user is not None:
+        _require_cuda_f32(user, "out")
+        if tuple(user.shape) != (n, c, oh, ow):
+            raise ValueError("out must have the pooled shape %r, got %r" % ((n, c, oh, ow), tuple(user.shape)))
+    pitch = slice_pitch(user) if user is not None else 0
+    direct = pitch >= c and pitch % 4 == 0 and user.data_ptr() % 16 == 0 and not _overlaps(x, user, pitch)
+    kout = user if direct else torch.empty((n, c, oh, ow), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+    with torch.cuda.device(x.device), _Timed("Pi" if direct and pitch != c else "P", kout.numel(), 4 + 4 * sh * sw):
+        L.check(L.load().fqb200_maxpool2d_nhwc_into(x.data_ptr(), kout.data_ptr(), n, h, w, c, kh, kw, sh, sw, ph, pw,
+                                                    pitch if direct else c, _stream_handle(x.device)))
+    return _finish_out(kout, None if direct else user)
 
 
 def _test_division(a, b):

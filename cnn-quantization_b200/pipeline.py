@@ -12,7 +12,7 @@ import torch.nn as nn
 
 from . import manager as M
 
-__all__ = ["CONFIGS", "build_quantized_model", "synthetic_batch", "validate", "accuracy_counts", "reduce_metrics", "HostFeeder"]
+__all__ = ["CONFIGS", "INPUT_SIZE", "ARCH_KWARGS", "build_quantized_model", "synthetic_batch", "validate", "accuracy_counts", "reduce_metrics", "HostFeeder"]
 
 # BASELINE.json configs -> reference CLI flags
 _W4A4 = dict(qtype="int4", qweight="int4", clipping="laplace", per_channel_quant_weights=True, per_channel_quant_act=True,
@@ -24,7 +24,16 @@ CONFIGS = {
     "vgg16_w4a4": dict(arch="vgg16", bit_alloc_target_act=5.3, bit_alloc_target_weight=5.3, **_W4A4),
     "vgg16_w4a4_mtq": dict(arch="vgg16", bit_alloc_target_act=5.3, bit_alloc_target_weight=5.3, mid_thread_quant=True, **_W4A4),
     "resnet18_w4a4": dict(arch="resnet18", **_W4A4),
+    # the paper's two remaining networks, "all methods combined" at 4W4A
+    "inception_v3_w4a4": dict(arch="inception_v3", **_W4A4),
+    "vgg16_bn_w4a4": dict(arch="vgg16_bn", **_W4A4),
 }
+# the square crop the reference's validation transform takes (inference_sim.py:217-218)
+INPUT_SIZE = {name: 299 if cfg["arch"] == "inception_v3" else 224 for name, cfg in CONFIGS.items()}
+# constructor keywords of the torchvision model, as ``pretrained=True`` builds it in the reference (the checkpoint itself is
+# not loaded).  Inception-v3's auxiliary head only runs in training, but its two convolutions and its linear take ids in
+# construction order and its weights are quantized, which the reference's max_mse_order_id (conv0..conv95) presumes.
+ARCH_KWARGS = {"inception_v3": dict(aux_logits=True, transform_input=True, init_weights=False)}
 
 
 def build_quantized_model(config, device, seed=12345, quantizer_factory=None, channels_last=False):
@@ -38,7 +47,7 @@ def build_quantized_model(config, device, seed=12345, quantizer_factory=None, ch
     qm.enable()
     try:
         torch.manual_seed(seed)  # inference_sim.py:127
-        model = models.__dict__[args.arch](weights=None)
+        model = models.__dict__[args.arch](weights=None, **ARCH_KWARGS.get(args.arch, {}))
     finally:
         qm.stop_stamping()
     M.set_node_names(model)
@@ -56,8 +65,11 @@ def build_quantized_model(config, device, seed=12345, quantizer_factory=None, ch
     return model, qm
 
 
-def synthetic_batch(batch, seed, device="cpu", hw=224, pin=False, channels_last=False):
-    """ImageNet-shaped input batch + labels; N(0,1) per pixel is what a normalised image roughly looks like."""
+def synthetic_batch(batch, seed, device="cpu", hw=None, pin=False, channels_last=False, config=None):
+    """ImageNet-shaped input batch + labels; N(0,1) per pixel is what a normalised image roughly looks like.  ``hw``
+    defaults to the crop of ``config`` (``INPUT_SIZE``), 224 without one."""
+    if hw is None:
+        hw = INPUT_SIZE.get(config, 224)
     g = torch.Generator().manual_seed(seed)
     x = torch.randn(batch, 3, hw, hw, generator=g)
     if channels_last:

@@ -219,11 +219,20 @@ int fqb200_quantize1_bca(const float* in, float* out, int64_t outer, int64_t gro
 /*
  * Max pooling of a channels-last activation ([n][h][w][c] in memory, c % 4 == 0; dilation 1, floor mode) - the operator in
  * front of the `activation_pooling` quantization call site (MaxPool2dWithId.forward, inference_quantization_manager.py:
- * 58-74).  out is [n][oh][ow][c], oh = (h + 2 ph - kh) / sh + 1.  Bit-identical to torch.nn.functional.max_pool2d
- * (NaN in a window wins).
+ * 58-74).  out is [n][oh][ow][c], oh = (h + 2 ph - kh) / sh + 1, and must not overlap in (FQB200_ERR_INVALID).
+ * Bit-identical to torch.nn.functional.max_pool2d (NaN in a window wins).
  */
 int fqb200_maxpool2d_nhwc(const float* in, float* out, int64_t n, int64_t h, int64_t w, int64_t c, int kh, int kw, int sh, int sw,
                           int ph, int pw, void* stream);
+/*
+ * fqb200_maxpool2d_nhwc writing a channel slice of a wider channels-last tensor: pixel p of the result goes to
+ * out + p * out_pixel_stride (out points at the slice's first channel); the other channels of every pixel are left
+ * untouched (the max-pool branch of an Inception block).  out_pixel_stride >= c and a multiple of 4, out 16-byte aligned
+ * (FQB200_ERR_UNSUPPORTED otherwise); out must not overlap in (FQB200_ERR_INVALID).  fqb200_maxpool2d_nhwc is the case
+ * out_pixel_stride = c, so it refuses overlapping tensors as well.
+ */
+int fqb200_maxpool2d_nhwc_into(const float* in, float* out, int64_t n, int64_t h, int64_t w, int64_t c, int kh, int kw,
+                               int sh, int sw, int ph, int pw, int64_t out_pixel_stride, void* stream);
 
 /*
  * out[i] = max(a[i] + b[i], 0) - the residual add + ReLU between two hooked convolutions of a ResNet block (the call
@@ -238,6 +247,19 @@ int fqb200_add_relu(const float* a, const float* b, float* out, int64_t n, void*
  */
 int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* workspace, size_t workspace_bytes,
                  void* stream);
+/*
+ * fqb200_fused writing its result into a channel slice of a wider channels-last tensor
+ * [outer][inner][out_pixel_stride]: pixel p of the result goes to out + p * out_pixel_stride (out points at the slice's
+ * first channel); the other channels of every pixel are left untouched.  A branch of an Inception block writes its part
+ * of the concatenation this way, bit for bit what fqb200_fused followed by a copy would give.
+ * Channels-last apply launches only (on-the-fly statistics, RANGE_GIVEN, torch and mid-tread leaves).
+ * FQB200_ERR_UNSUPPORTED: stats_only, pool, residual or a non-channels-last descriptor; out_pixel_stride < groups or not
+ * a multiple of 4; a misaligned in / out.  out_pixel_stride = groups is the dense case, where `out` may alias `in`; with
+ * any other pitch an `out` overlapping `in` returns FQB200_ERR_INVALID.  These rules are checked before any device call.
+ * fqb200_fused(d, ...) is fqb200_fused_into(d, ..., 0, ...): a dense `out` for any descriptor.
+ */
+int fqb200_fused_into(const fqb200_desc* d, const float* in, float* out, int64_t out_pixel_stride, void* workspace,
+                      size_t workspace_bytes, void* stream);
 
 /*
  * KL-divergence calibration (`-kld` collect, statistic_manager.py:80-82 -> kld_threshold.py:15-80): for each of `rows`
