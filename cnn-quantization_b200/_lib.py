@@ -23,7 +23,8 @@ SYMBOLS = ("fqb200_abi_version", "fqb200_last_error", "fqb200_resident_ctas", "f
            "fqb200_maxpool2d_nhwc", "fqb200_maxpool2d_nhwc_into",
            "fqb200_kld_threshold", "fqb200_kld_workspace_bytes", "fqb200_sample_sumsq",
            "fqb200_sample_sumsq_workspace_bytes", "fqb200_clip_error", "fqb200_clip_error_workspace_bytes",
-           "fqb200_kmeans1d", "fqb200_kmeans1d_workspace_bytes")
+           "fqb200_kmeans1d", "fqb200_kmeans1d_workspace_bytes", "fqb200_sample_angles",
+           "fqb200_sample_angles_workspace_bytes")
 ABI_VERSION = 3
 
 
@@ -107,6 +108,10 @@ def load():
     lib.fqb200_sample_sumsq.argtypes = [vp, i64, i64, vp, vp, ctypes.c_size_t, vp]
     lib.fqb200_sample_sumsq_workspace_bytes.restype = ctypes.c_size_t
     lib.fqb200_sample_sumsq_workspace_bytes.argtypes = [i64, i64]
+    lib.fqb200_sample_angles.restype = i32
+    lib.fqb200_sample_angles.argtypes = [vp, i64, i64, vp, vp, vp, ctypes.c_size_t, i32, vp]
+    lib.fqb200_sample_angles_workspace_bytes.restype = ctypes.c_size_t
+    lib.fqb200_sample_angles_workspace_bytes.argtypes = [i64, i64]
     lib.fqb200_clip_error.restype = i32
     lib.fqb200_clip_error.argtypes = [vp, i64, i64, i64, i32, vp, i32, i32, i32, i32, vp, vp, vp, ctypes.c_size_t, i32, vp]
     lib.fqb200_clip_error_workspace_bytes.restype = ctypes.c_size_t

@@ -1104,6 +1104,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_measure.cuh"
 #include "fq_cliperr.cuh"
 #include "fq_kmeans.cuh"
+#include "fq_angle.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1290,6 +1291,7 @@ struct DeviceInfo {
   int resident_cl[2] = {0, 0};  // channels-last kernels without / with the histogram
   int resident_bca = 0;         // fq_cl_bca_kernel
   int resident_rows = 0;        // fq_rows_kernel
+  int resident_angle[2] = {0, 0};  // fq_gram_partial_kernel<1>, <4>
 };
 constexpr int kMaxDevices = 64;
 constexpr int kAssumedSms = 132;  // H100 SXM: the SM count plans assume when no device is present
@@ -1424,6 +1426,15 @@ void init_device(int dev) {
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kBulkThreads, cl_given_smem());
     if (e != cudaSuccess || n < 1) return bad("row kernel setup", e);
     d.resident_rows = sms * n;
+  }
+  for (int v = 0; v < 2; ++v) {
+    int n = 0;
+    const void* fn = v ? reinterpret_cast<const void*>(fqb::fq_gram_partial_kernel<4>)
+                       : reinterpret_cast<const void*>(fqb::fq_gram_partial_kernel<1>);
+    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(fqb::kAngSmemBytes));
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kAngThreads, fqb::kAngSmemBytes);
+    if (e != cudaSuccess || n < 1) return bad("Gram kernel setup", e);
+    d.resident_angle[v] = sms * n;
   }
   const void* given[4] = {reinterpret_cast<const void*>(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, false>),
                           reinterpret_cast<const void*>(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, true>),
@@ -1650,6 +1661,12 @@ size_t sumsq_workspace(int64_t rows, int64_t row_len) {
   const unsigned long long chunk = fqb::sumsq_chunk(static_cast<unsigned long long>(row_len));
   const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
   return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * 8 : 0;
+}
+
+// sample-angle workspace: one 64 x 64 float64 block per (tile pair, slice) unit (fq_angle.cuh)
+size_t angle_workspace(int64_t rows, int64_t row_len) {
+  const fqb::AngleSplit s = fqb::angle_split(static_cast<unsigned long long>(rows), static_cast<unsigned long long>(row_len));
+  return static_cast<size_t>(s.pairs * s.slices) * fqb::kAngTile * fqb::kAngTile * 8;
 }
 
 // clipping-error workspace: kCeSums float64 partials per (group, unit) (fq_cliperr.cuh)
@@ -2433,6 +2450,62 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch sum-of-squares kernels: %s", cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+// the requests fqb200_sample_angles takes (FQB200_OK, or the code with the message in fqb200_last_error())
+static int angle_bad_args(int64_t rows, int64_t row_len) {
+  if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s");
+  if (rows > fqb::kAngMaxRows) return fail(FQB200_ERR_UNSUPPORTED, "rows must be <= 8192%s");
+  return FQB200_OK;
+}
+
+size_t fqb200_sample_angles_workspace_bytes(int64_t rows, int64_t row_len) {
+  g_err[0] = 0;
+  if (angle_bad_args(rows, row_len) != FQB200_OK) return 0;
+  return angle_workspace(rows, row_len);
+}
+
+int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* out_angles, double* out_gram,
+                         void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  int rc = angle_bad_args(rows, row_len);
+  if (rc != FQB200_OK) return rc;
+  if (!out_angles && !out_gram) return fail(FQB200_ERR_INVALID, "null pointer: out_angles and out_gram%s");
+  if (!in) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  const size_t need = angle_workspace(rows, row_len);
+  if (need && (!workspace || workspace_bytes < need || !aligned16(workspace)))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_sample_angles_workspace_bytes() or not 16-byte aligned%s");
+  if (rows == 0) return FQB200_OK;
+  DeviceInfo* di = nullptr;
+  rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const fqb::AngleSplit sp = fqb::angle_split(static_cast<unsigned long long>(rows), static_cast<unsigned long long>(row_len));
+  fqb::AngleArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.rows = static_cast<unsigned long long>(rows);
+  A.row_len = static_cast<unsigned long long>(row_len);
+  A.tiles = sp.tiles;
+  A.pairs = sp.pairs;
+  A.slices = sp.slices;
+  A.slice_steps = sp.slice_steps;
+  A.partial = static_cast<double*>(workspace);
+  A.angles = out_angles;
+  A.gram = out_gram;
+  const bool vec = row_len % 4 == 0 && aligned16(in);
+  const unsigned long long units = A.pairs * A.slices;
+  const unsigned long long cap = max_ctas ? static_cast<unsigned long long>(max_ctas)
+                                          : static_cast<unsigned long long>(di->resident_angle[vec ? 1 : 0]);
+  const int grid = static_cast<int>(units < cap ? units : cap);
+  if (vec) fqb::fq_gram_partial_kernel<4><<<grid, fqb::kAngThreads, fqb::kAngSmemBytes, st>>>(A);
+  else     fqb::fq_gram_partial_kernel<1><<<grid, fqb::kAngThreads, fqb::kAngSmemBytes, st>>>(A);
+  const dim3 fgrid(fqb::kAngTile * fqb::kAngTile / fqb::kAngFinishThreads, static_cast<unsigned>(A.pairs));
+  fqb::fq_gram_finish_kernel<<<fgrid, fqb::kAngFinishThreads, 0, st>>>(A);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch Gram kernels: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
 

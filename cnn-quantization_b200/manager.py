@@ -31,15 +31,17 @@ FUSED_RELU_ARCHS = ("alexnet", "vgg16", "vgg16_bn", "inception_v3")
 
 def make_args(**over):
     """An ``args`` namespace with the reference CLI's defaults (inference/inference_sim.py:52-112) for the fields the
-    manager and the quantizers read.  Extensions without a reference flag: ``stats_base_dir`` and ``collect_err`` (fill the
-    mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument)."""
+    manager and the quantizers read.  Extensions without a reference flag: ``stats_base_dir``, ``collect_err`` (fill the
+    mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument) and
+    ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms, or "angle", the
+    pairwise sample angles of its angle_stats module, which the reference selects by editing an import)."""
     d = dict(arch="resnet18", qtype=None, qweight="int8", q_off=False, clipping="no", stats_mode="no", stats_kind="mean",
              stats_folder=None, stats_batch_avg=False, kld_threshold=False, measure_stats=False,
              per_channel_quant_weights=False, per_channel_quant_act=False, bit_alloc_act=False, bit_alloc_weight=False,
              bit_alloc_rmode="round", bit_alloc_prior="gaus", bit_alloc_target_act=None, bit_alloc_target_weight=None,
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
              mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
-             collect_err=False)
+             collect_err=False, measure_stats_kind="distance")
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -377,12 +379,16 @@ class QuantizationManagerInference(object):
         # max(q + identity, 0), a deferred shortcut is quantized only inside the consuming launch, a pooling launch writes
         # the pooled quarter - so they are switched off; each is bit-identical to its unfused form.
         self.measure_stats = None
+        kind = getattr(args, "measure_stats_kind", "distance")
+        if kind not in ("distance", "angle"):
+            raise ValueError("measure_stats_kind must be 'distance' or 'angle', got %r" % (kind,))
         if args.measure_stats:
             import torch.distributed as dist
             if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
                 raise NotImplementedError("-ms with several ranks: per-rank shards would put the rows out of sample order")
-            from .statistics import MeasureStatistics
-            self.measure_stats = MeasureStatistics(args.arch, getattr(args, "stats_base_dir", None))
+            from .statistics import AngleStatistics, MeasureStatistics
+            cls = AngleStatistics if kind == "angle" else MeasureStatistics
+            self.measure_stats = cls(args.arch, getattr(args, "stats_base_dir", None))
             self.fuse_residual_into_quant = self.defer_shortcut = self.fuse_pool_into_quant = False
             self.fuse_inception_concat = False   # the hooked output is the tensor -ms measures; keep torch.cat's
         # `collect_err`: the collect hooks hand each tensor's use-mode quantizer settings to save_tensor_stats, which fills
@@ -531,7 +537,7 @@ class QuantizationManagerInference(object):
         if self.stats_manager is not None:
             self.stats_manager.__exit__()  # collect mode: write the CSV / pickle files
         if self.measure_stats is not None:
-            self.measure_stats.__exit__()  # -ms: write distance.csv
+            self.measure_stats.__exit__()  # -ms: write distance.csv (angle.pkl with the angle kind)
 
     # -- call sites: forward hooks reproducing the *WithId.forward bodies (:58-74, :84-101, :162-217, :227-250, :262-283)
     def attach(self, model):

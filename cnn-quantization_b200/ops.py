@@ -24,8 +24,8 @@ def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
-    (ops.sample_sumsq), 'E' the clipping-error measurement (ops.clip_error) and 'C' the k-means clustering of a weight
-    tensor (ops.kmeans1d), which quantize nothing."""
+    (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'E' the clipping-error measurement
+    (ops.clip_error) and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -506,6 +506,38 @@ def sample_sumsq(x):
         L.check(lib.fqb200_sample_sumsq(x.data_ptr(), rows, row_len, out.data_ptr(), ws.data_ptr() if ws is not None else None,
                                         need, _stream_handle(dev)))
     return out
+
+
+def sample_angles(x, return_gram=False, max_ctas=0):
+    """C ABI fqb200_sample_angles: the pairwise angles between the samples (dim 0) of ``x`` as a float32 [N, N] device
+    tensor - ``acos(cos_sim(x[i], x[j]))`` for j > i and 0 on and below the diagonal, the matrix the reference's angle
+    measurement records (angle_stats.py:29-37).  The cosine comes from the float64 Gram matrix (FP64 tensor cores), is
+    clamped to [-1, 1] (the reference's fp32 cosine can step over 1 and give NaN) and is NaN where it is not finite (a zero
+    sample, NaN / Inf input).  With ``return_gram`` also returns the float64 [N, N] Gram matrix (valid for j >= i).
+    Deterministic (the bits depend neither on the run nor on ``max_ctas``), no host synchronisation.  Recorded in the launch
+    profile under mode 'G' (one read of the tensor)."""
+    _require_cuda_f32(x, "tensor")
+    if x.dim() == 0:
+        raise ValueError("sample_angles needs a tensor with a sample dimension")
+    if not dense(x):
+        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    dev = x.device
+    rows = x.shape[0]
+    angles = torch.empty((rows, rows), dtype=torch.float32, device=dev)
+    gram = torch.empty((rows, rows), dtype=torch.float64, device=dev) if return_gram else None
+    if rows > 0:
+        if x.numel() == 0:
+            raise ValueError("sample_angles needs samples of at least one element")
+        lib = L.load()
+        row_len = x.numel() // rows
+        need = lib.fqb200_sample_angles_workspace_bytes(rows, row_len)
+        ws = torch.empty(need, dtype=torch.uint8, device=dev) if need else None
+        with torch.cuda.device(dev), _Timed("G", x.numel(), 4, "%dx%d" % (rows, row_len)):
+            L.check(lib.fqb200_sample_angles(x.data_ptr(), rows, row_len, angles.data_ptr(),
+                                             gram.data_ptr() if gram is not None else None,
+                                             ws.data_ptr() if ws is not None else None, need, int(max_ctas),
+                                             _stream_handle(dev)))
+    return (angles, gram) if return_gram else angles
 
 
 CLIP_ERROR_CANDIDATES = ("lowp", "gaus", "laplace")

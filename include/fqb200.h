@@ -292,6 +292,31 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
 size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len);
 
 /*
+ * Sample-angle measurement (angle_stats.py:17-44): for `rows` contiguous rows of `row_len` floats (one sample; any dense
+ * memory order of it), the float64 Gram matrix G = X X^T on the FP64 tensor cores (fp32 products are exact in float64,
+ * accumulation in float64) and the pairwise angles.  Outputs, row-major [rows][rows]:
+ *   out_angles (float32): float(acos(c_ij)) for j > i with c_ij = G_ij / sqrt(G_ii * G_jj) in float64, clamped to
+ *     [-1, 1]; 0 on and below the diagonal.  A pair whose cosine is not finite is NaN: a zero sample (0 / 0, as in the
+ *     reference) and a sample holding NaN or Inf.  The clamp differs from the reference on purpose: its fp32 cosine can
+ *     land a rounding step above 1 for nearly parallel samples and give NaN.  A duplicated sample gives exactly 0 and a
+ *     negated one exactly float(pi).
+ *   out_gram (float64, may be null): G_ij for j >= i; the entries below the diagonal are unspecified.
+ * At least one of the two outputs must be given.  rows <= 8192 (FQB200_ERR_UNSUPPORTED above); rows == 0 launches nothing.
+ * The reduction is cut into K slices whose count depends on (rows, row_len) only; each (64 x 64 tile pair, slice) unit
+ * writes its partial to its own workspace slot and a second launch adds them in slice order, so the bits do not depend on
+ * the run or on max_ctas (0: the default grid, else at most that many CTAs).  Two launches on `stream`, no host
+ * synchronisation.  The workspace (fqb200_sample_angles_workspace_bytes, 16-byte aligned; at most (P + 1024) * 32 KB
+ * with P = T (T + 1) / 2 tile pairs, T = ceil(rows / 64): 34 MB at rows = 512) is private to the call.
+ * FQB200_ERR_INVALID: rows < 0, row_len <= 0, max_ctas < 0, `in` or both outputs null; FQB200_ERR_WORKSPACE: a workspace
+ * that is missing, too small or misaligned.
+ */
+int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* out_angles, double* out_gram,
+                         void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream);
+/* Workspace of fqb200_sample_angles in bytes (0 and fqb200_last_error() on bad arguments: rows < 0, row_len <= 0,
+ * rows > 8192). */
+size_t fqb200_sample_angles_workspace_bytes(int64_t rows, int64_t row_len);
+
+/*
  * Clipping-error measurement (the mse_* / cos_* columns of `-sm collect`, statistic_manager.py:83-111): for every group g
  * of x (layout as fqb200_desc: outer x groups x inner, NCHW order; or channels_last != 0: [outer][inner][groups] memory,
  * groups % 4 == 0, 4 <= groups <= 2048) and the three candidate quantizers of get_alpha(clip_type='mix')
