@@ -16,15 +16,6 @@ PRIOR_STD, PRIOR_B = 0, 1
 STATS_STRIDE = 12
 STAT_COLUMNS = ("min", "max", "mean", "b", "std", "delta", "offset", "bits", "scale", "zero_point", "qmax", "flags")
 
-# every symbol include/fqb200.h declares (tests check the export table against this)
-SYMBOLS = ("fqb200_abi_version", "fqb200_last_error", "fqb200_resident_ctas", "fqb200_plan_info",
-           "fqb200_selftest_division", "fqb200_workspace_bytes", "fqb200_workspace_init", "fqb200_float2gemmlowp",
-           "fqb200_quantize1", "fqb200_quantize1_bca", "fqb200_fused", "fqb200_fused_into", "fqb200_add_relu",
-           "fqb200_maxpool2d_nhwc", "fqb200_maxpool2d_nhwc_into",
-           "fqb200_kld_threshold", "fqb200_kld_workspace_bytes", "fqb200_sample_sumsq",
-           "fqb200_sample_sumsq_workspace_bytes", "fqb200_clip_error", "fqb200_clip_error_workspace_bytes",
-           "fqb200_kmeans1d", "fqb200_kmeans1d_workspace_bytes", "fqb200_sample_angles",
-           "fqb200_sample_angles_workspace_bytes")
 ABI_VERSION = 3
 
 
@@ -55,6 +46,40 @@ class Desc(ctypes.Structure):
     ]
 
 
+_vp, _i64, _i32, _f32, _sz, _desc = (ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float, ctypes.c_size_t,
+                                      ctypes.POINTER(Desc))
+# name -> (restype, argtypes) of every function include/fqb200.h declares (tests check the export table against this)
+PROTOTYPES = {
+    "fqb200_abi_version": (_i32, []),
+    "fqb200_last_error": (ctypes.c_char_p, []),
+    "fqb200_resident_ctas": (_i32, []),
+    "fqb200_plan_info": (_i32, [_desc, ctypes.POINTER(ctypes.c_int64)]),
+    "fqb200_selftest_division": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp]),
+    "fqb200_workspace_bytes": (_sz, [_desc]),
+    "fqb200_workspace_init": (_i32, [_vp, _sz, _vp]),
+    "fqb200_float2gemmlowp": (_i32, [_vp, _vp, _i64, _f32, _f32, _i32, _i32, _i32, _vp, _vp]),
+    "fqb200_quantize1": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _vp]),
+    "fqb200_quantize1_bca": (_i32, [_vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _sz, _vp]),
+    "fqb200_fused": (_i32, [_desc, _vp, _vp, _vp, _sz, _vp]),
+    "fqb200_fused_into": (_i32, [_desc, _vp, _vp, _i64, _vp, _sz, _vp]),
+    "fqb200_add_relu": (_i32, [_vp, _vp, _vp, _i64, _vp]),
+    "fqb200_maxpool2d_nhwc": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "fqb200_maxpool2d_nhwc_into": (_i32, [_vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _vp]),
+    "fqb200_kld_threshold": (_i32, [_vp, _i64, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "fqb200_kld_workspace_bytes": (_sz, [_i64, _i32]),
+    "fqb200_sample_sumsq": (_i32, [_vp, _i64, _i64, _vp, _vp, _sz, _vp]),
+    "fqb200_sample_sumsq_workspace_bytes": (_sz, [_i64, _i64]),
+    "fqb200_clip_error": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _i32, _vp]),
+    "fqb200_clip_error_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32]),
+    "fqb200_kmeans1d": (_i32, [_vp, _i64, _i32, _i64, _vp, _i32, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                               _i32, _vp]),
+    "fqb200_kmeans1d_workspace_bytes": (_sz, [_i64, _i32]),
+    "fqb200_sample_angles": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp, _sz, _i32, _vp]),
+    "fqb200_sample_angles_workspace_bytes": (_sz, [_i64, _i64]),
+}
+SYMBOLS = tuple(PROTOTYPES)
+
+
 class FqError(RuntimeError):
     pass
 
@@ -71,58 +96,9 @@ def load():
         raise FqError("libfqb200.so is not built (run `python cnn-quantization_b200/build.py` or "
                       "__graft_entry__.build()); there is no CPU fallback for the fake-quantization path")
     lib = ctypes.CDLL(LIB_PATH)
-    vp, i64, i32, f32 = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_float
-    lib.fqb200_abi_version.restype = i32
-    lib.fqb200_abi_version.argtypes = []
-    lib.fqb200_last_error.restype = ctypes.c_char_p
-    lib.fqb200_last_error.argtypes = []
-    lib.fqb200_resident_ctas.restype = i32
-    lib.fqb200_resident_ctas.argtypes = []
-    lib.fqb200_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_workspace_bytes.argtypes = [ctypes.POINTER(Desc)]
-    lib.fqb200_workspace_init.restype = i32
-    lib.fqb200_workspace_init.argtypes = [vp, ctypes.c_size_t, vp]
-    lib.fqb200_float2gemmlowp.restype = i32
-    lib.fqb200_float2gemmlowp.argtypes = [vp, vp, i64, f32, f32, i32, i32, i32, vp, vp]
-    lib.fqb200_quantize1.restype = i32
-    lib.fqb200_quantize1.argtypes = [vp, vp, vp, i64, i64, i64, vp, vp, vp, i32, i32, vp, i32, vp]
-    lib.fqb200_fused.restype = i32
-    lib.fqb200_fused.argtypes = [ctypes.POINTER(Desc), vp, vp, vp, ctypes.c_size_t, vp]
-    lib.fqb200_fused_into.restype = i32
-    lib.fqb200_fused_into.argtypes = [ctypes.POINTER(Desc), vp, vp, i64, vp, ctypes.c_size_t, vp]
-    lib.fqb200_quantize1_bca.restype = i32
-    lib.fqb200_quantize1_bca.argtypes = [vp, vp, i64, i64, i64, vp, vp, vp, i32, i32, vp, i32, vp, vp, ctypes.c_size_t, vp]
-    lib.fqb200_maxpool2d_nhwc.restype = i32
-    lib.fqb200_maxpool2d_nhwc.argtypes = [vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, i32, vp]
-    lib.fqb200_maxpool2d_nhwc_into.restype = i32
-    lib.fqb200_maxpool2d_nhwc_into.argtypes = [vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, i32, i64, vp]
-    lib.fqb200_add_relu.restype = i32
-    lib.fqb200_add_relu.argtypes = [vp, vp, vp, i64, vp]
-    lib.fqb200_selftest_division.restype = i32
-    lib.fqb200_selftest_division.argtypes = [vp, vp, vp, vp, i64, vp]
-    lib.fqb200_kld_threshold.restype = i32
-    lib.fqb200_kld_threshold.argtypes = [vp, i64, i64, i32, i32, vp, vp, vp, vp, ctypes.c_size_t, vp]
-    lib.fqb200_kld_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_kld_workspace_bytes.argtypes = [i64, i32]
-    lib.fqb200_sample_sumsq.restype = i32
-    lib.fqb200_sample_sumsq.argtypes = [vp, i64, i64, vp, vp, ctypes.c_size_t, vp]
-    lib.fqb200_sample_sumsq_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_sample_sumsq_workspace_bytes.argtypes = [i64, i64]
-    lib.fqb200_sample_angles.restype = i32
-    lib.fqb200_sample_angles.argtypes = [vp, i64, i64, vp, vp, vp, ctypes.c_size_t, i32, vp]
-    lib.fqb200_sample_angles_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_sample_angles_workspace_bytes.argtypes = [i64, i64]
-    lib.fqb200_clip_error.restype = i32
-    lib.fqb200_clip_error.argtypes = [vp, i64, i64, i64, i32, vp, i32, i32, i32, i32, vp, vp, vp, ctypes.c_size_t, i32, vp]
-    lib.fqb200_clip_error_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_clip_error_workspace_bytes.argtypes = [i64, i64, i64, i32]
-    lib.fqb200_kmeans1d.restype = i32
-    lib.fqb200_kmeans1d.argtypes = [vp, i64, i32, i64, vp, i32, vp, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, ctypes.c_size_t,
-                                    i32, vp]
-    lib.fqb200_kmeans1d_workspace_bytes.restype = ctypes.c_size_t
-    lib.fqb200_kmeans1d_workspace_bytes.argtypes = [i64, i32]
-    lib.fqb200_plan_info.restype = i32
-    lib.fqb200_plan_info.argtypes = [ctypes.POINTER(Desc), ctypes.POINTER(ctypes.c_int64)]
+    for name, (restype, argtypes) in PROTOTYPES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.fqb200_abi_version() != ABI_VERSION:
         raise FqError("libfqb200.so ABI version mismatch")
     _lib = lib

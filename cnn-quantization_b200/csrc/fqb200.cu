@@ -1267,6 +1267,37 @@ int fail(int code, const char* fmt, const char* detail = "", const char* detail2
   return code;
 }
 
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// `need` bytes of caller workspace, as `sizer`() reports them (none: anything goes)
+int check_workspace(const void* ws, size_t bytes, size_t need, const char* sizer) {
+  if (need && (!ws || bytes < need || !aligned16(ws)))
+    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than %s() or not 16-byte aligned", sizer);
+  return FQB200_OK;
+}
+
+// the error of the launches just queued, if any
+int launched(const char* what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) return FQB200_OK;
+  return fail(FQB200_ERR_CUDA, *what ? "launch %s: %s" : "launch%s: %s", what, cudaGetErrorString(e));
+}
+
+// one CTA per work unit, at most `cap`, or at most `max_ctas` when the caller sets it
+int grid_for(unsigned long long units, unsigned long long cap, int max_ctas = 0) {
+  if (max_ctas > 0) cap = static_cast<unsigned long long>(max_ctas);
+  return static_cast<int>(units < cap ? units : cap);
+}
+
+// allow `fn` `smem` bytes of dynamic shared memory; with `per_sm`, also count its CTAs of `threads` that fit on an SM
+template <class F>
+cudaError_t setup(F fn, int threads, size_t smem, int* per_sm = nullptr) {
+  const void* f = reinterpret_cast<const void*>(fn);
+  cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e == cudaSuccess && per_sm) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, f, threads, smem);
+  return e;
+}
+
 // channels-last kernel variants: leaf (torch / mid-tread) x second statistics pass x histogram
 const void* cl_kernel_ptr(int leaf, bool dev, bool hist) {
 #define FQB_CL(L, D, H) reinterpret_cast<const void*>(fqb::fq_cl_kernel<L, D, H>)
@@ -1345,6 +1376,25 @@ double laplace_opt_alpha(double w) {
   return a;
 }
 
+// KLD kernels (fq_kld.cuh): shared-memory histogram replicas, and the dynamic shared memory of the histogram and search
+// kernels
+constexpr int kKldMaxBins = 8001;
+int kld_replicas(int num_bins) {
+  const int rep = 65536 / (num_bins * 4);
+  return rep < 1 ? 1 : (rep > fqb::kKldMaxReplicas ? fqb::kKldMaxReplicas : rep);
+}
+size_t kld_hist_smem(int num_bins) { return static_cast<size_t>(kld_replicas(num_bins) + 1) * num_bins * 4 + 4; }
+size_t kld_search_smem(int num_bins) {
+  return static_cast<size_t>((2 * (num_bins + 1) + 1) & ~1) * 4 + static_cast<size_t>(num_bins / 2 + 1) * 8;
+}
+
+size_t kmeans_smem(int k) {
+  const size_t stage = static_cast<size_t>(fqb::kKmMaxT) * fqb::kKmBlk * 8;
+  const size_t acc = static_cast<size_t>(fqb::kWarps) * k * 12;
+  const size_t tot = static_cast<size_t>(fqb::kThreads) * 16;
+  return stage > acc ? (stage > tot ? stage : tot) : (acc > tot ? acc : tot);
+}
+
 // One-time, per-device set-up (kernel attributes, occupancy, constant tables).  Runs under std::call_once: the reference's
 // callers include torch.nn.DataParallel worker threads, one per device (SURVEY 8b).
 void init_device(int dev) {
@@ -1363,18 +1413,13 @@ void init_device(int dev) {
         for (int cr = 0; cr < 2; ++cr) {
           if (modes[mi] == 8 && cr) continue;
           int n = 0;
-          const void* fn = fused_kernel_ptr(modes[mi], leaf, dv != 0, cr != 0);
-          const int smem = static_cast<int>(dyn_smem(modes[mi] == 1 ? 1 : 4));
-          e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-          if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kThreads, smem);
+          e = setup(fused_kernel_ptr(modes[mi], leaf, dv != 0, cr != 0), fqb::kThreads, dyn_smem(modes[mi] == 1 ? 1 : 4), &n);
           if (e != cudaSuccess) return bad("fused kernel setup", e);
           if (n < per_sm) per_sm = n;
         }
   {
     int n = 0;
-    const void* fn = reinterpret_cast<const void*>(fqb::fq_fused_kernel<4, FQB200_LEAF_COMPILED, false, false, true>);
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn_smem(4)));
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kThreads, dyn_smem(4));
+    e = setup(fqb::fq_fused_kernel<4, FQB200_LEAF_COMPILED, false, false, true>, fqb::kThreads, dyn_smem(4), &n);
     if (e != cudaSuccess) return bad("bias-period kernel setup", e);
     if (n < per_sm) per_sm = n;
   }
@@ -1388,10 +1433,7 @@ void init_device(int dev) {
     for (int leaf = 0; leaf < 3; leaf += 2)
       for (int dv = 0; dv < 2; ++dv) {
         int n = 0;
-        const void* fn = cl_kernel_ptr(leaf, dv != 0, hist != 0);
-        const size_t smem = cl_smem(hist != 0);
-        e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kBulkThreads, smem);
+        e = setup(cl_kernel_ptr(leaf, dv != 0, hist != 0), fqb::kBulkThreads, cl_smem(hist != 0), &n);
         if (e != cudaSuccess && hist) {  // the histogram variant may not fit next to an enlarged ring (development builds)
           (void)cudaGetLastError();
           n = 0;
@@ -1411,49 +1453,35 @@ void init_device(int dev) {
     }
     d.resident_cl[hist] = sms * worst;
   }
-  {
-    int n = 0;
-    const void* fn = reinterpret_cast<const void*>(fqb::fq_cl_bca_kernel);
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cl_smem(false)));
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kBulkThreads, cl_smem(false));
-    if (e != cudaSuccess || n < 1) return bad("bias-correction kernel setup", e);
-    d.resident_bca = sms * n;
-  }
-  {
-    int n = 0;
-    const void* fn = reinterpret_cast<const void*>(fqb::fq_rows_kernel);
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cl_given_smem()));
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kBulkThreads, cl_given_smem());
-    if (e != cudaSuccess || n < 1) return bad("row kernel setup", e);
-    d.resident_rows = sms * n;
-  }
+  int n = 0;
+  e = setup(fqb::fq_cl_bca_kernel, fqb::kBulkThreads, cl_smem(false), &n);
+  if (e != cudaSuccess || n < 1) return bad("bias-correction kernel setup", e);
+  d.resident_bca = sms * n;
+  e = setup(fqb::fq_rows_kernel, fqb::kBulkThreads, cl_given_smem(), &n);
+  if (e != cudaSuccess || n < 1) return bad("row kernel setup", e);
+  d.resident_rows = sms * n;
   for (int v = 0; v < 2; ++v) {
-    int n = 0;
-    const void* fn = v ? reinterpret_cast<const void*>(fqb::fq_gram_partial_kernel<4>)
-                       : reinterpret_cast<const void*>(fqb::fq_gram_partial_kernel<1>);
-    e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(fqb::kAngSmemBytes));
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, fqb::kAngThreads, fqb::kAngSmemBytes);
+    e = setup(v ? fqb::fq_gram_partial_kernel<4> : fqb::fq_gram_partial_kernel<1>, fqb::kAngThreads, fqb::kAngSmemBytes, &n);
     if (e != cudaSuccess || n < 1) return bad("Gram kernel setup", e);
     d.resident_angle[v] = sms * n;
   }
-  const void* given[4] = {reinterpret_cast<const void*>(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, false>),
-                          reinterpret_cast<const void*>(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, true>),
-                          reinterpret_cast<const void*>(fqb::fq_cl_given_kernel<false>),
-                          reinterpret_cast<const void*>(fqb::fq_cl_given_kernel<true>)};
-  for (int i = 0; i < 4; ++i) {
-    e = cudaFuncSetAttribute(given[i], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             static_cast<int>(i < 2 ? dyn_smem(4) : cl_given_smem()));
-    if (e != cudaSuccess) return bad("given-parameter kernel setup", e);
-  }
-  e = cudaFuncSetAttribute(reinterpret_cast<const void*>(fqb::fq_cl_given_fused_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           static_cast<int>(cl_given_smem()));
+  if ((e = setup(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, false>, fqb::kThreads, dyn_smem(4))) != cudaSuccess ||
+      (e = setup(fqb::fq_given_kernel<4, FQB200_LEAF_TORCH, true>, fqb::kThreads, dyn_smem(4))) != cudaSuccess ||
+      (e = setup(fqb::fq_cl_given_kernel<false>, fqb::kBulkThreads, cl_given_smem())) != cudaSuccess ||
+      (e = setup(fqb::fq_cl_given_kernel<true>, fqb::kBulkThreads, cl_given_smem())) != cudaSuccess)
+    return bad("given-parameter kernel setup", e);
+  e = setup(fqb::fq_cl_given_fused_kernel, fqb::kBulkThreads, cl_given_smem());
   if (e != cudaSuccess) return bad("given-parameter fused kernel setup", e);
-  const void* leafb[2] = {reinterpret_cast<const void*>(fqb::fq_leaf_bulk_kernel<false>),
-                          reinterpret_cast<const void*>(fqb::fq_leaf_bulk_kernel<true>)};
-  for (int i = 0; i < 2; ++i) {
-    e = cudaFuncSetAttribute(leafb[i], cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cl_given_smem()));
-    if (e != cudaSuccess) return bad("a1 bulk kernel setup", e);
-  }
+  if ((e = setup(fqb::fq_leaf_bulk_kernel<false>, fqb::kBulkThreads, cl_given_smem())) != cudaSuccess ||
+      (e = setup(fqb::fq_leaf_bulk_kernel<true>, fqb::kBulkThreads, cl_given_smem())) != cudaSuccess)
+    return bad("a1 bulk kernel setup", e);
+  // the KLD and k-means launches size their shared memory by argument: allow the largest any accepted argument needs
+  if ((e = setup(fqb::fq_kld_hist_kernel<1>, fqb::kKldThreads, kld_hist_smem(kKldMaxBins))) != cudaSuccess ||
+      (e = setup(fqb::fq_kld_hist_kernel<4>, fqb::kKldThreads, kld_hist_smem(kKldMaxBins))) != cudaSuccess ||
+      (e = setup(fqb::fq_kld_search_kernel, fqb::kKldThreads, kld_search_smem(kKldMaxBins))) != cudaSuccess)
+    return bad("KLD kernel setup", e);
+  e = setup(fqb::fq_kmeans_kernel, fqb::kThreads, kmeans_smem(fqb::kKmMaxK));
+  if (e != cudaSuccess) return bad("k-means kernel setup", e);
   // mid-tread table (int_quantizer.py:41-51): omega grid = 5 decades x 20 steps, leading 0
   double om[fqb::kTable], al[fqb::kTable];
   om[0] = 0.0;
@@ -1491,8 +1519,6 @@ struct Plan {
   int mode;  // 4, 1, 8 (bundled 128-bit path) or 2 (flat stream on the bulk-copy engine)
   int grid;
 };
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 constexpr uint64_t kUnitsPerCta = 8;  // dynamic work units per resident CTA
 
@@ -1554,7 +1580,7 @@ int make_plan(int64_t outer, int64_t groups, int64_t inner, bool can_vec, bool a
   g.row_pitch = G * inner_v;
   pl->vec = vec;
   pl->mode = mode;
-  pl->grid = static_cast<int>(units < ctas ? units : ctas);
+  pl->grid = grid_for(units, ctas);
   return FQB200_OK;
 }
 
@@ -1590,7 +1616,7 @@ int make_plan_flat(uint64_t elems, int64_t channels, int max_ctas, Plan* pl) {
   pl->geo.channels = g.channels;  // solve_bit_alloc reads the channel count here
   pl->vec = 4;
   pl->mode = 2;
-  pl->grid = static_cast<int>(units < ctas ? units : ctas);
+  pl->grid = grid_for(units, ctas);
   return FQB200_OK;
 }
 
@@ -1631,7 +1657,7 @@ int make_plan_rows(uint64_t rows, uint64_t row_elems, int64_t channels, int max_
   pl->geo.channels = static_cast<unsigned>(rows);
   pl->vec = 4;
   pl->mode = 3;
-  pl->grid = static_cast<int>(units < ctas ? units : ctas);
+  pl->grid = grid_for(units, ctas);
   return FQB200_OK;
 }
 
@@ -1715,13 +1741,6 @@ size_t kmeans_carve(char* base, unsigned long long n, int k, fqb::KmArgs* A) {
   }
   return off;
 }
-size_t kmeans_smem(int k) {
-  const size_t stage = static_cast<size_t>(fqb::kKmMaxT) * fqb::kKmBlk * 8;
-  const size_t acc = static_cast<size_t>(fqb::kWarps) * k * 12;
-  const size_t tot = static_cast<size_t>(fqb::kThreads) * 16;
-  return stage > acc ? (stage > tot ? stage : tot) : (acc > tot ? acc : tot);
-}
-
 // workspace layout; returns total bytes, fills pointers when base != nullptr.  Partials: one slot per unit.
 size_t carve(char* base, uint64_t slots, uint64_t groups, fqb::FusedArgs* A) {
   size_t off = 0;
@@ -2000,12 +2019,14 @@ int plan_fused(const fqb200_desc* d, bool can_vec, int64_t out_pitch, const Devi
   return FQB200_OK;
 }
 
-// the resident-CTA counts plans are made for without a launch: the current device's, or an H100's when there is none
+// the resident-CTA counts plans are made for without a launch: the current device's, or, when there is none, an H100's
+// at each kernel family's __launch_bounds__ residency
 DeviceInfo plan_residency() {
   DeviceInfo* di = nullptr;
   if (get_device(&di) == FQB200_OK) return *di;
   DeviceInfo h;
-  h.resident = h.resident_cl[0] = h.resident_cl[1] = h.resident_rows = kAssumedSms * fqb::kCtasPerSm;
+  h.resident = kAssumedSms * fqb::kCtasPerSm;
+  h.resident_cl[0] = h.resident_cl[1] = h.resident_rows = kAssumedSms * fqb::kBulkCtasPerSm;
   return h;
 }
 
@@ -2106,14 +2127,10 @@ int fqb200_float2gemmlowp(const float* in, float* out, int64_t n, float range, f
     B.q = q;
     if (noise) fqb::fq_leaf_bulk_kernel<true><<<pl.grid, fqb::kBulkThreads, cl_given_smem(), st>>>(B);
     else       fqb::fq_leaf_bulk_kernel<false><<<pl.grid, fqb::kBulkThreads, cl_given_smem(), st>>>(B);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_leaf_bulk_kernel: %s", cudaGetErrorString(e));
-    return FQB200_OK;
+    return launched("fq_leaf_bulk_kernel");
   }
   const unsigned long long nvec = vec ? static_cast<unsigned long long>(n / 4) : static_cast<unsigned long long>(n);
-  unsigned long long want = (nvec + fqb::kThreads * 4ull - 1) / (fqb::kThreads * 4ull);
-  const unsigned long long cap = static_cast<unsigned long long>(di->resident) * 2ull;
-  const int grid = static_cast<int>(want < cap ? want : cap);
+  const int grid = grid_for((nvec + fqb::kThreads * 4ull - 1) / (fqb::kThreads * 4ull), di->resident * 2ull);
   const float as = fabsf(q.a);
   const bool fast = (as > 1e-30f) && (as < 1e30f);
 #define FQB_LAUNCH_LEAF(V, N, F) fqb::fq_leaf_kernel<V, N, F><<<grid, fqb::kThreads, 0, st>>>(in, out, noise, nvec, q)
@@ -2125,9 +2142,7 @@ int fqb200_float2gemmlowp(const float* in, float* out, int64_t n, float range, f
     else       { if (fast) FQB_LAUNCH_LEAF(1, false, true); else FQB_LAUNCH_LEAF(1, false, false); }
   }
 #undef FQB_LAUNCH_LEAF
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_leaf_kernel: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("fq_leaf_kernel");
 }
 
 int fqb200_quantize1(const float* in, float* out, float* grid, int64_t outer, int64_t groups, int64_t inner,
@@ -2171,9 +2186,7 @@ int fqb200_quantize1(const float* in, float* out, float* grid, int64_t outer, in
     A.flat = pl.flat;
     if (grid) fqb::fq_cl_given_kernel<true><<<pl.grid, fqb::kBulkThreads, cl_given_smem(), st>>>(A);
     else      fqb::fq_cl_given_kernel<false><<<pl.grid, fqb::kBulkThreads, cl_given_smem(), st>>>(A);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_cl_given_kernel: %s", cudaGetErrorString(e));
-    return FQB200_OK;
+    return launched("fq_cl_given_kernel");
   }
   rc = make_plan(outer, groups, inner, can_vec, false, di->resident * 2, &pl);
   if (rc != FQB200_OK) return rc;
@@ -2185,9 +2198,7 @@ int fqb200_quantize1(const float* in, float* out, float* grid, int64_t outer, in
     if (grid) fqb::fq_given_kernel<1, FQB200_LEAF_TORCH, true><<<pl.grid, fqb::kThreads, dyn_smem(1), st>>>(A);
     else      fqb::fq_given_kernel<1, FQB200_LEAF_TORCH, false><<<pl.grid, fqb::kThreads, dyn_smem(1), st>>>(A);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_given_kernel: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("fq_given_kernel");
 }
 
 int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* workspace, size_t workspace_bytes,
@@ -2222,11 +2233,9 @@ int fqb200_fused_into(const fqb200_desc* d, const float* in, float* out, int64_t
   FusedPlan fp;
   rc = plan_fused(d, can_vec, out_pixel_stride == d->groups ? 0 : out_pixel_stride, *di, &fp);   // pitch C: dense
   if (rc != FQB200_OK) return rc;
-  if (fp.workspace) {
-    if (!workspace || workspace_bytes < fp.workspace) return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_workspace_bytes()%s");
-    if (!aligned16(workspace)) return fail(FQB200_ERR_WORKSPACE, "workspace must be 16-byte aligned%s");
-    carve(static_cast<char*>(workspace), fp.slots, fp.pl.geo.channels, &fp.A);
-  }
+  rc = check_workspace(workspace, workspace_bytes, fp.workspace, "fqb200_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  if (fp.workspace) carve(static_cast<char*>(workspace), fp.slots, fp.pl.geo.channels, &fp.A);
   fp.A.in = in;
   fp.A.out = out;
   void* args[] = {&fp.A};
@@ -2248,16 +2257,17 @@ int fqb200_quantize1_bca(const float* in, float* out, int64_t outer, int64_t gro
   if (bits && !per_group) return fail(FQB200_ERR_INVALID, "per-row bit widths need per-group parameters%s");
   if (!(aligned16(in) && aligned16(out) && flat_eligible(groups)))
     return fail(FQB200_ERR_UNSUPPORTED, "bias-corrected quantization runs on channels-last tensors: 16-byte aligned, C %% 4 == 0, C <= 2048%s");
+  int rc = check_workspace(workspace, workspace_bytes, carve(nullptr, 0, static_cast<uint64_t>(groups), nullptr),
+                           "fqb200_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   DeviceInfo* di = nullptr;
-  int rc = get_device(&di);
+  rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   Plan pl;
   rc = make_plan_flat(static_cast<uint64_t>(outer) * groups * inner, groups, di->resident_bca, &pl);
   if (rc != FQB200_OK) return rc;
   fqb::FusedArgs A;
   memset(&A, 0, sizeof(A));
-  const size_t need = carve(nullptr, 0, static_cast<uint64_t>(groups), nullptr);
-  if (!workspace || workspace_bytes < need) return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_workspace_bytes()%s");
   carve(static_cast<char*>(workspace), 0, static_cast<uint64_t>(groups), &A);
   A.flat = pl.flat;
   A.geo = pl.geo;
@@ -2311,13 +2321,9 @@ int fqb200_maxpool2d_nhwc_into(const float* in, float* out, int64_t n, int64_t h
   P.oh = static_cast<unsigned>(oh); P.ow = static_cast<unsigned>(ow);
   P.kh = kh; P.kw = kw; P.sh = sh; P.sw = sw; P.ph = ph; P.pw = pw;
   P.total = static_cast<unsigned long long>(n) * oh * ow * (c / 4);
-  unsigned long long want = (P.total + 255ull) / 256ull;
-  const unsigned long long cap = static_cast<unsigned long long>(di->sms) * 32ull;
-  const int grid = static_cast<int>(want < cap ? want : cap);
+  const int grid = grid_for((P.total + 255ull) / 256ull, di->sms * 32ull);
   fqb::fq_maxpool_nhwc_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(P);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_maxpool_nhwc_kernel: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("fq_maxpool_nhwc_kernel");
 }
 
 int fqb200_add_relu(const float* a, const float* b, float* out, int64_t n, void* stream) {
@@ -2331,37 +2337,33 @@ int fqb200_add_relu(const float* a, const float* b, float* out, int64_t n, void*
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool vec = (n % 4 == 0) && aligned16(a) && aligned16(b) && aligned16(out);
   const unsigned long long nvec = vec ? static_cast<unsigned long long>(n / 4) : static_cast<unsigned long long>(n);
-  unsigned long long want = (nvec + fqb::kThreads * 4ull - 1) / (fqb::kThreads * 4ull);
-  const unsigned long long cap = static_cast<unsigned long long>(di->resident) * 4ull;
-  const int grid = static_cast<int>(want < cap ? want : cap);
+  const int grid = grid_for((nvec + fqb::kThreads * 4ull - 1) / (fqb::kThreads * 4ull), di->resident * 4ull);
   if (vec) fqb::fq_add_relu_kernel<4><<<grid, fqb::kThreads, 0, st>>>(a, b, out, nvec);
   else     fqb::fq_add_relu_kernel<1><<<grid, fqb::kThreads, 0, st>>>(a, b, out, nvec);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch fq_add_relu_kernel: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("fq_add_relu_kernel");
 }
 
 size_t fqb200_kld_workspace_bytes(int64_t rows, int num_bins) {
   g_err[0] = 0;
   if (rows <= 0 || rows > (1ll << 31) - 1) return fail(FQB200_ERR_INVALID, "rows must be in 1 .. 2^31 - 1%s"), 0;
-  if (num_bins < 3 || num_bins > 8001 || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s"), 0;
+  if (num_bins < 3 || num_bins > kKldMaxBins || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s"), 0;
   return kld_workspace(rows, num_bins);
 }
 
 int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num_bins, int num_quantized_bins, float* out_th,
                          float* out_div, int32_t* out_idx, void* workspace, size_t workspace_bytes, void* stream) {
   g_err[0] = 0;
-  if (num_bins < 3 || num_bins > 8001 || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s");
+  if (num_bins < 3 || num_bins > kKldMaxBins || num_bins % 2 == 0) return fail(FQB200_ERR_INVALID, "num_bins must be odd, 3 .. 8001%s");
   if (num_quantized_bins < 3 || num_quantized_bins > num_bins || num_quantized_bins % 2 == 0)
     return fail(FQB200_ERR_INVALID, "num_quantized_bins must be odd, 3 .. num_bins%s");
   if (rows <= 0 || row_len <= 0 || rows > (1ll << 31) - 1) return fail(FQB200_ERR_INVALID, "rows / row_len must be positive (rows < 2^31)%s");
   if (row_len > (1ll << 31) - 1) return fail(FQB200_ERR_UNSUPPORTED, "rows of 2^31 elements and more (int32 bin counts)%s");
   if (!in || !out_th || !out_div || !out_idx) return fail(FQB200_ERR_INVALID, "null pointer%s");
   const size_t need = kld_workspace(rows, num_bins);
-  if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15u))
-    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_kld_workspace_bytes() or not 16-byte aligned%s");
+  int rc = check_workspace(workspace, workspace_bytes, need, "fqb200_kld_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   DeviceInfo* di = nullptr;
-  int rc = get_device(&di);
+  rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   fqb::KldArgs A;
@@ -2380,24 +2382,15 @@ int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num
   A.hist = reinterpret_cast<unsigned*>(static_cast<char*>(workspace) + align_up(static_cast<size_t>(rows) * 4, 256));
   A.nb = num_bins;
   A.nq = num_quantized_bins;
-  int rep = 65536 / (num_bins * 4);
-  A.replicas = rep < 1 ? 1 : (rep > fqb::kKldMaxReplicas ? fqb::kKldMaxReplicas : rep);
+  A.replicas = kld_replicas(num_bins);
   A.out_th = out_th;
   A.out_div = out_div;
   A.out_idx = out_idx;
-  const size_t hist_smem = static_cast<size_t>(A.replicas + 1) * num_bins * 4 + 4;
-  const size_t search_smem = static_cast<size_t>((2 * (num_bins + 1) + 1) & ~1) * 4 + static_cast<size_t>(num_bins / 2 + 1) * 8;
+  const size_t hist_smem = kld_hist_smem(num_bins), search_smem = kld_search_smem(num_bins);
   const bool vec = row_len % 4 == 0 && aligned16(in);
-  const void* hist_k = vec ? reinterpret_cast<const void*>(fqb::fq_kld_hist_kernel<4>) : reinterpret_cast<const void*>(fqb::fq_kld_hist_kernel<1>);
-  cudaError_t e = cudaFuncSetAttribute(hist_k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(hist_smem));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(reinterpret_cast<const void*>(fqb::fq_kld_search_kernel), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             static_cast<int>(search_smem));
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaFuncSetAttribute (KLD kernels): %s", cudaGetErrorString(e));
-  e = cudaMemsetAsync(workspace, 0, need, st);
+  const cudaError_t e = cudaMemsetAsync(workspace, 0, need, st);
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaMemsetAsync: %s", cudaGetErrorString(e));
-  const unsigned long long units = A.rows * A.chunks;
-  const int grid = static_cast<int>(units < want ? units : want);
+  const int grid = grid_for(A.rows * A.chunks, want);
   if (vec) {
     fqb::fq_kld_absmax_kernel<4><<<grid, fqb::kKldThreads, 0, st>>>(A);
     fqb::fq_kld_hist_kernel<4><<<grid, fqb::kKldThreads, hist_smem, st>>>(A);
@@ -2406,9 +2399,7 @@ int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num
     fqb::fq_kld_hist_kernel<1><<<grid, fqb::kKldThreads, hist_smem, st>>>(A);
   }
   fqb::fq_kld_search_kernel<<<static_cast<unsigned>(rows), fqb::kKldThreads, search_smem, st>>>(A);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch KLD kernels: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("KLD kernels");
 }
 
 size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len) {
@@ -2422,12 +2413,11 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
   g_err[0] = 0;
   if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s");
   if (!in || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
-  const size_t need = sumsq_workspace(rows, row_len);
-  if (need && (!workspace || workspace_bytes < need || !aligned16(workspace)))
-    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_sample_sumsq_workspace_bytes() or not 16-byte aligned%s");
+  int rc = check_workspace(workspace, workspace_bytes, sumsq_workspace(rows, row_len), "fqb200_sample_sumsq_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   if (rows == 0) return FQB200_OK;
   DeviceInfo* di = nullptr;
-  int rc = get_device(&di);
+  rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   fqb::SumsqArgs A;
@@ -2439,18 +2429,14 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
   A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
   A.partial = static_cast<double*>(workspace);
   A.out = out;
-  const unsigned long long units = A.rows * A.chunks;
-  const unsigned long long cap = static_cast<unsigned long long>(di->sms) * (2048ull / fqb::kSumsqThreads);
-  const int grid = static_cast<int>(units < cap ? units : cap);
+  const int grid = grid_for(A.rows * A.chunks, di->sms * (2048ull / fqb::kSumsqThreads));
   if (row_len % 4 == 0 && aligned16(in)) fqb::fq_sumsq_partial_kernel<4><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
   else                                   fqb::fq_sumsq_partial_kernel<1><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
   if (A.chunks > 1) {
     const unsigned long long blocks = (A.rows + fqb::kSumsqThreads - 1) / fqb::kSumsqThreads;
     fqb::fq_sumsq_finish_kernel<<<static_cast<unsigned>(blocks), fqb::kSumsqThreads, 0, st>>>(A);
   }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch sum-of-squares kernels: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("sum-of-squares kernels");
 }
 
 // the requests fqb200_sample_angles takes (FQB200_OK, or the code with the message in fqb200_last_error())
@@ -2474,9 +2460,8 @@ int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* 
   if (!out_angles && !out_gram) return fail(FQB200_ERR_INVALID, "null pointer: out_angles and out_gram%s");
   if (!in) return fail(FQB200_ERR_INVALID, "null pointer%s");
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
-  const size_t need = angle_workspace(rows, row_len);
-  if (need && (!workspace || workspace_bytes < need || !aligned16(workspace)))
-    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_sample_angles_workspace_bytes() or not 16-byte aligned%s");
+  rc = check_workspace(workspace, workspace_bytes, angle_workspace(rows, row_len), "fqb200_sample_angles_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   if (rows == 0) return FQB200_OK;
   DeviceInfo* di = nullptr;
   rc = get_device(&di);
@@ -2496,17 +2481,12 @@ int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* 
   A.angles = out_angles;
   A.gram = out_gram;
   const bool vec = row_len % 4 == 0 && aligned16(in);
-  const unsigned long long units = A.pairs * A.slices;
-  const unsigned long long cap = max_ctas ? static_cast<unsigned long long>(max_ctas)
-                                          : static_cast<unsigned long long>(di->resident_angle[vec ? 1 : 0]);
-  const int grid = static_cast<int>(units < cap ? units : cap);
+  const int grid = grid_for(A.pairs * A.slices, di->resident_angle[vec ? 1 : 0], max_ctas);
   if (vec) fqb::fq_gram_partial_kernel<4><<<grid, fqb::kAngThreads, fqb::kAngSmemBytes, st>>>(A);
   else     fqb::fq_gram_partial_kernel<1><<<grid, fqb::kAngThreads, fqb::kAngSmemBytes, st>>>(A);
   const dim3 fgrid(fqb::kAngTile * fqb::kAngTile / fqb::kAngFinishThreads, static_cast<unsigned>(A.pairs));
   fqb::fq_gram_finish_kernel<<<fgrid, fqb::kAngFinishThreads, 0, st>>>(A);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch Gram kernels: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("Gram kernels");
 }
 
 // the layouts fqb200_clip_error takes (argument errors as a message, nullptr when they are fine)
@@ -2535,11 +2515,11 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
   if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
   if (bit_alloc && num_bits > 4) return fail(FQB200_ERR_INVALID, "bit_alloc applies to num_bits <= 4 only%s");
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
-  const size_t need = cliperr_workspace(outer, groups, inner, channels_last);
-  if (!workspace || workspace_bytes < need || !aligned16(workspace))
-    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_clip_error_workspace_bytes() or not 16-byte aligned%s");
+  int rc = check_workspace(workspace, workspace_bytes, cliperr_workspace(outer, groups, inner, channels_last),
+                           "fqb200_clip_error_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   DeviceInfo* di = nullptr;
-  int rc = get_device(&di);
+  rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   fqb::ClipErrArgs A;
@@ -2559,15 +2539,11 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
   A.partial = static_cast<double*>(workspace);
   A.out = out;
   A.params = out_params;
-  const unsigned long long cap = max_ctas ? static_cast<unsigned long long>(max_ctas)
-                                          : static_cast<unsigned long long>(di->sms) * (2048ull / fqb::kCeThreads);
-  const int grid = static_cast<int>(A.units < cap ? A.units : cap);
+  const int grid = grid_for(A.units, di->sms * (2048ull / fqb::kCeThreads), max_ctas);
   if (!channels_last && inner % 4 == 0 && aligned16(in)) fqb::fq_cliperr_partial_kernel<4><<<grid, fqb::kCeThreads, 0, st>>>(A);
   else                                                   fqb::fq_cliperr_partial_kernel<1><<<grid, fqb::kCeThreads, 0, st>>>(A);
   fqb::fq_cliperr_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCeThreads, 0, st>>>(A);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch clipping-error kernels: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("clipping-error kernels");
 }
 
 // the requests fqb200_kmeans1d takes (argument errors as a message, nullptr when they are fine)
@@ -2610,10 +2586,10 @@ int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_
   fqb::KmArgs A;
   memset(&A, 0, sizeof(A));
   const size_t need = kmeans_carve(static_cast<char*>(workspace), static_cast<unsigned long long>(n), k, &A);
-  if (!workspace || workspace_bytes < need || !aligned16(workspace))
-    return fail(FQB200_ERR_WORKSPACE, "workspace smaller than fqb200_kmeans1d_workspace_bytes() or not 16-byte aligned%s");
+  int rc = check_workspace(workspace, workspace_bytes, need, "fqb200_kmeans1d_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
   DeviceInfo* di = nullptr;
-  int rc = get_device(&di);
+  rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   A.in = in;
@@ -2634,17 +2610,16 @@ int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_
   const void* fn = reinterpret_cast<const void*>(fqb::fq_kmeans_kernel);
   const size_t smem = kmeans_smem(k);
   int per_sm = 0;
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, fqb::kThreads, smem);
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, fqb::kThreads, smem);
   if (e != cudaSuccess || per_sm < 1) return fail(FQB200_ERR_CUDA, "k-means kernel setup: %s", cudaGetErrorString(e));
-  const long long resident = static_cast<long long>(di->sms) * per_sm;
-  const long long grid = max_ctas && max_ctas < resident ? max_ctas : resident;
+  const unsigned long long resident = static_cast<unsigned long long>(di->sms) * per_sm;
+  const int grid = grid_for(resident, resident, max_ctas);
   // barrier words and control block start at zero
   e = cudaMemsetAsync(workspace, 0, reinterpret_cast<char*>(A.col) - static_cast<char*>(workspace), st);
   if (e == cudaSuccess && init && out_init_ids) e = cudaMemsetAsync(out_init_ids, 0xff, static_cast<size_t>(k) * 8, st);
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaMemsetAsync: %s", cudaGetErrorString(e));
   void* args[] = {&A};
-  e = cudaLaunchCooperativeKernel(fn, dim3(static_cast<unsigned>(grid)), dim3(fqb::kThreads), args, smem, st);
+  e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(fqb::kThreads), args, smem, st);
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_kmeans_kernel: %s", cudaGetErrorString(e));
   return FQB200_OK;
 }
@@ -2652,9 +2627,7 @@ int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_
 int fqb200_selftest_division(const float* a, const float* b, float* fast, float* ieee, int64_t n, void* stream) {
   if (n <= 0) return FQB200_OK;
   fqb::fq_divtest_kernel<<<296, 256, 0, static_cast<cudaStream_t>(stream)>>>(a, b, fast, ieee, static_cast<unsigned long long>(n));
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "launch: %s", cudaGetErrorString(e));
-  return FQB200_OK;
+  return launched("");
 }
 
 }  // extern "C"

@@ -71,6 +71,17 @@ def _require_cuda_f32(t, name):
         raise TypeError("%s must be float32, got %s" % (name, t.dtype))
 
 
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _launch(dev, timed, fn, *args):
+    """``fn(*args, stream)`` on the current stream of ``dev``, recorded in the launch profile by ``timed`` (a ``_Timed``);
+    raises on an error code."""
+    with torch.cuda.device(dev), timed:
+        L.check(fn(*args, _stream_handle(dev)))
+
+
 def _workspace(device, stream, nbytes):
     key = (device.index, stream)
     ws = _workspaces.get(key)
@@ -80,6 +91,27 @@ def _workspace(device, stream, nbytes):
         L.check(L.load().fqb200_workspace_init(ws.data_ptr(), ws.numel(), stream))
         _workspaces[key] = ws
     return ws
+
+
+def _own_workspace(device, need, required=True):
+    """A workspace for one launch that zeroes or fills it itself (the shared ``_workspace`` keeps the fused kernels'
+    barriers): ``need`` bytes as the entry point's sizer reports them, None for 0.  ``required``: 0 is the sizer refusing
+    the arguments; raise its error."""
+    if not need and required:
+        L.check(L.ERR_INVALID)
+    return torch.empty(need, dtype=torch.uint8, device=device) if need else None
+
+
+def _samples(x, what):
+    """(x, rows, row_len) of a float32 CUDA tensor read sample by sample (dim 0).  A sample is contiguous in NCHW and in
+    channels-last memory; anything else is copied."""
+    _require_cuda_f32(x, "tensor")
+    if x.dim() == 0:
+        raise ValueError("%s needs a tensor with a sample dimension" % what)
+    if not dense(x):
+        x = x.contiguous()
+    rows = x.shape[0]
+    return x, rows, (x.numel() // rows if rows else 0)
 
 
 def nhwc(x):
@@ -201,10 +233,8 @@ def float2gemmlowp(x, range_, offset, num_bits, int_exp, enforce_true_zero, nois
         x = x.contiguous()
         noise = noise.contiguous() if noise is not None else None
     kout, uout = _resolve_out(x, out)
-    with torch.cuda.device(x.device), _Timed("A", x.numel(), 8):
-        L.check(lib.fqb200_float2gemmlowp(x.data_ptr(), kout.data_ptr(), x.numel(), float(range_), float(offset),
-                                          int(num_bits), int(bool(int_exp)), int(bool(enforce_true_zero)),
-                                          noise.data_ptr() if noise is not None else None, _stream_handle(x.device)))
+    _launch(x.device, _Timed("A", x.numel(), 8), lib.fqb200_float2gemmlowp, x.data_ptr(), kout.data_ptr(), x.numel(),
+            float(range_), float(offset), int(num_bits), int(bool(int_exp)), int(bool(enforce_true_zero)), _ptr(noise))
     return _finish_out(kout, uout)
 
 
@@ -243,11 +273,9 @@ def quantize1(x, delta, offset, num_bits, bits=None, layout=None, want_grid=Fals
             raise ValueError("bias must have one element per group (%d)" % groups)
     kout, uout = _resolve_out(x, out)
     grid = torch.empty_like(x) if want_grid else None
-    with torch.cuda.device(dev), _Timed("A", x.numel(), 8, "%dx%dx%d" % (outer, groups, inner)):
-        L.check(lib.fqb200_quantize1(x.data_ptr(), kout.data_ptr(), grid.data_ptr() if want_grid else None,
-                                     outer, groups, inner, delta.data_ptr(), offset.data_ptr(),
-                                     bits.data_ptr() if bits is not None else None, int(per_group), int(num_bits),
-                                     bias.data_ptr() if bias is not None else None, int(cl), _stream_handle(dev)))
+    _launch(dev, _Timed("A", x.numel(), 8, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_quantize1, x.data_ptr(),
+            kout.data_ptr(), _ptr(grid), outer, groups, inner, delta.data_ptr(), offset.data_ptr(), _ptr(bits),
+            int(per_group), int(num_bits), _ptr(bias), int(cl))
     out = _finish_out(kout, uout)
     return (out, grid) if want_grid else out
 
@@ -279,13 +307,10 @@ def quantize1_bca(x, delta, offset, num_bits, bits=None, bias=None, relu_first=F
     d = L.Desc()
     d.outer, d.groups, d.inner, d.num_bits, d.channels_last = n, c, inner, 8, 1
     with torch.cuda.device(dev):
-        stream = _stream_handle(dev)
-        ws = _workspace(dev, stream, lib.fqb200_workspace_bytes(ctypes.byref(d)))
-        with _Timed("C", x.numel(), 12, "%dx%dx%d" % (n, c, inner)):
-            L.check(lib.fqb200_quantize1_bca(x.data_ptr(), kout.data_ptr(), n, c, inner, delta.data_ptr(), offset.data_ptr(),
-                                             bits.data_ptr() if bits is not None else None, int(per_group), int(num_bits),
-                                             bias.data_ptr() if bias is not None else None, int(bool(relu_first)),
-                                             qb.data_ptr() if qb is not None else None, ws.data_ptr(), ws.numel(), stream))
+        ws = _workspace(dev, _stream_handle(dev), lib.fqb200_workspace_bytes(ctypes.byref(d)))
+    _launch(dev, _Timed("C", x.numel(), 12, "%dx%dx%d" % (n, c, inner)), lib.fqb200_quantize1_bca, x.data_ptr(),
+            kout.data_ptr(), n, c, inner, delta.data_ptr(), offset.data_ptr(), _ptr(bits), int(per_group), int(num_bits),
+            _ptr(bias), int(bool(relu_first)), _ptr(qb), ws.data_ptr(), ws.numel())
     res = _finish_out(kout, uout)
     return (res, qb) if want_qbias else res
 
@@ -420,26 +445,24 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     else:
         kout, uout = _resolve_out(x, out)
     with torch.cuda.device(dev):
-        stream = _stream_handle(dev)
         need = lib.fqb200_workspace_bytes(ctypes.byref(d))
         if need == 0:
             L.check(L.ERR_INVALID)
-        ws = _workspace(dev, stream, need)
-        two_pass = (range_mode != L.RANGE_MINMAX or leaf == L.LEAF_MIDTREAD or var_corr or stats_only or
-                    (bit_alloc and num_bits <= 4 and scope == L.SCOPE_GROUP))
-        mode = "S" if stats_only else ("D" if two_pass else "B")
-        bpe = (8 if two_pass else 4) + (0 if stats_only else 8)
-        if range_mode == L.RANGE_GIVEN:
-            mode, bpe = "A", 8
-        if residual is not None:   # + the residual read of the fused block epilogue (the write is the apply's own)
-            mode, bpe = mode + "r", bpe + 4
-        if pooled is not None:     # the apply phase reads x (3x3: rows twice, the second time mostly out of L2) and writes a quarter
-            mode, bpe = mode + "p", bpe - 3
-        if pitch:                  # written into a channel slice of a wider tensor
-            mode += "i"
-        with _Timed(mode, x.numel(), bpe, "%dx%dx%d" % (outer, groups, inner)):
-            L.check(lib.fqb200_fused_into(ctypes.byref(d), x.data_ptr(), kout.data_ptr() if kout is not None else None,
-                                          pitch, ws.data_ptr(), ws.numel(), stream))
+        ws = _workspace(dev, _stream_handle(dev), need)
+    two_pass = (range_mode != L.RANGE_MINMAX or leaf == L.LEAF_MIDTREAD or var_corr or stats_only or
+                (bit_alloc and num_bits <= 4 and scope == L.SCOPE_GROUP))
+    mode = "S" if stats_only else ("D" if two_pass else "B")
+    bpe = (8 if two_pass else 4) + (0 if stats_only else 8)
+    if range_mode == L.RANGE_GIVEN:
+        mode, bpe = "A", 8
+    if residual is not None:   # + the residual read of the fused block epilogue (the write is the apply's own)
+        mode, bpe = mode + "r", bpe + 4
+    if pooled is not None:     # the apply phase reads x (3x3: rows twice, the second time mostly out of L2) and writes a quarter
+        mode, bpe = mode + "p", bpe - 3
+    if pitch:                  # written into a channel slice of a wider tensor
+        mode += "i"
+    _launch(dev, _Timed(mode, x.numel(), bpe, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_fused_into, ctypes.byref(d),
+            x.data_ptr(), _ptr(kout), pitch, ws.data_ptr(), ws.numel())
     if stats_only:
         return stats
     if pooled is not None:
@@ -455,28 +478,17 @@ def kld_threshold(x, num_bins=2001, num_quantized_bins=15, return_hist=False):
     (int32); a sample holding NaN / Inf gets NaN, NaN, -1.  With ``return_hist`` the [N, num_bins] int32 bin counts come
     fourth (a view of the workspace).  Recorded in the launch profile under mode 'K' (two reads of the tensor), apart from
     the quantization launches."""
-    _require_cuda_f32(x, "tensor")
-    if x.dim() == 0:
-        raise ValueError("kld_threshold needs a tensor with a sample dimension")
-    if not dense(x):
-        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    x, rows, row_len = _samples(x, "kld_threshold")
     lib = L.load()
     dev = x.device
-    rows = x.shape[0]
     th = torch.empty(rows, dtype=torch.float32, device=dev)
     div = torch.empty(rows, dtype=torch.float32, device=dev)
     idx = torch.empty(rows, dtype=torch.int32, device=dev)
     if rows == 0:
         return (th, div, idx, torch.zeros((0, num_bins), dtype=torch.int32, device=dev)) if return_hist else (th, div, idx)
-    row_len = x.numel() // rows
-    need = lib.fqb200_kld_workspace_bytes(rows, int(num_bins))
-    if need == 0:
-        L.check(L.ERR_INVALID)
-    # a workspace of its own: the launch zeroes it and fills it with counters (the fused kernels' workspace keeps barriers)
-    ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev), _Timed("K", x.numel(), 8, "%dx%d" % (rows, row_len)):
-        L.check(lib.fqb200_kld_threshold(x.data_ptr(), rows, row_len, int(num_bins), int(num_quantized_bins), th.data_ptr(),
-                                         div.data_ptr(), idx.data_ptr(), ws.data_ptr(), ws.numel(), _stream_handle(dev)))
+    ws = _own_workspace(dev, lib.fqb200_kld_workspace_bytes(rows, int(num_bins)))
+    _launch(dev, _Timed("K", x.numel(), 8, "%dx%d" % (rows, row_len)), lib.fqb200_kld_threshold, x.data_ptr(), rows, row_len,
+            int(num_bins), int(num_quantized_bins), th.data_ptr(), div.data_ptr(), idx.data_ptr(), ws.data_ptr(), ws.numel())
     if not return_hist:
         return th, div, idx
     head = (rows * 4 + 255) // 256 * 256   # the counters follow the rows' max |x| words (fqb200_kld_threshold)
@@ -488,23 +500,16 @@ def sample_sumsq(x):
     tensor - the activation norm `-ms` records (distance_stats.py:27-28).  Deterministic (fixed chunks, fixed summation
     order), no host synchronisation.  Recorded in the launch profile under mode 'M' (one read of the tensor), apart from
     the quantization launches."""
-    _require_cuda_f32(x, "tensor")
-    if x.dim() == 0:
-        raise ValueError("sample_sumsq needs a tensor with a sample dimension")
-    if not dense(x):
-        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    x, rows, row_len = _samples(x, "sample_sumsq")
     dev = x.device
-    rows = x.shape[0]
     if rows == 0 or x.numel() == 0:
         return torch.zeros(rows, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
     lib = L.load()
-    row_len = x.numel() // rows
     out = torch.empty(rows, dtype=torch.float64, device=dev)
     need = lib.fqb200_sample_sumsq_workspace_bytes(rows, row_len)
-    ws = torch.empty(need, dtype=torch.uint8, device=dev) if need else None
-    with torch.cuda.device(dev), _Timed("M", x.numel(), 4, "%dx%d" % (rows, row_len)):
-        L.check(lib.fqb200_sample_sumsq(x.data_ptr(), rows, row_len, out.data_ptr(), ws.data_ptr() if ws is not None else None,
-                                        need, _stream_handle(dev)))
+    ws = _own_workspace(dev, need, required=False)
+    _launch(dev, _Timed("M", x.numel(), 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_sumsq, x.data_ptr(), rows, row_len,
+            out.data_ptr(), _ptr(ws), need)
     return out
 
 
@@ -516,27 +521,18 @@ def sample_angles(x, return_gram=False, max_ctas=0):
     sample, NaN / Inf input).  With ``return_gram`` also returns the float64 [N, N] Gram matrix (valid for j >= i).
     Deterministic (the bits depend neither on the run nor on ``max_ctas``), no host synchronisation.  Recorded in the launch
     profile under mode 'G' (one read of the tensor)."""
-    _require_cuda_f32(x, "tensor")
-    if x.dim() == 0:
-        raise ValueError("sample_angles needs a tensor with a sample dimension")
-    if not dense(x):
-        x = x.contiguous()   # a sample is contiguous in NCHW and in channels-last memory; anything else is copied
+    x, rows, row_len = _samples(x, "sample_angles")
     dev = x.device
-    rows = x.shape[0]
     angles = torch.empty((rows, rows), dtype=torch.float32, device=dev)
     gram = torch.empty((rows, rows), dtype=torch.float64, device=dev) if return_gram else None
     if rows > 0:
         if x.numel() == 0:
             raise ValueError("sample_angles needs samples of at least one element")
         lib = L.load()
-        row_len = x.numel() // rows
         need = lib.fqb200_sample_angles_workspace_bytes(rows, row_len)
-        ws = torch.empty(need, dtype=torch.uint8, device=dev) if need else None
-        with torch.cuda.device(dev), _Timed("G", x.numel(), 4, "%dx%d" % (rows, row_len)):
-            L.check(lib.fqb200_sample_angles(x.data_ptr(), rows, row_len, angles.data_ptr(),
-                                             gram.data_ptr() if gram is not None else None,
-                                             ws.data_ptr() if ws is not None else None, need, int(max_ctas),
-                                             _stream_handle(dev)))
+        ws = _own_workspace(dev, need, required=False)
+        _launch(dev, _Timed("G", x.numel(), 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_angles, x.data_ptr(), rows,
+                row_len, angles.data_ptr(), _ptr(gram), _ptr(ws), need, int(max_ctas))
     return (angles, gram) if return_gram else angles
 
 
@@ -576,15 +572,10 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
     if x.numel() == 0:
         out.zero_()
         return (out, params) if want_params else out
-    need = lib.fqb200_clip_error_workspace_bytes(outer, groups, inner, int(bool(channels_last)))
-    if need == 0:
-        L.check(L.ERR_INVALID)
-    ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev), _Timed("E", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)):
-        L.check(lib.fqb200_clip_error(x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(),
-                                      int(num_bits), int(bool(positive)), int(bool(bit_alloc)), int(bool(solve_f64)),
-                                      out.data_ptr(), params.data_ptr() if params is not None else None, ws.data_ptr(), need,
-                                      int(max_ctas), _stream_handle(dev)))
+    ws = _own_workspace(dev, lib.fqb200_clip_error_workspace_bytes(outer, groups, inner, int(bool(channels_last))))
+    _launch(dev, _Timed("E", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_error, x.data_ptr(), outer,
+            groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), int(bool(bit_alloc)),
+            int(bool(solve_f64)), out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
     return (out, params) if want_params else out
 
 
@@ -656,16 +647,11 @@ def kmeans1d(x, num_bits, seed=0, task=None, init=None, rows=None, max_ctas=0):
         init_t = torch.as_tensor(init, dtype=torch.float64).reshape(-1).to(dev).contiguous()
         if init_t.numel() != k:
             raise ValueError("init must hold %d centres" % k)
-    need = lib.fqb200_kmeans1d_workspace_bytes(n, k)
-    if need == 0:
-        L.check(L.ERR_INVALID)
-    ws = torch.empty(need, dtype=torch.uint8, device=dev)
-    ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
-    with torch.cuda.device(dev), _Timed("C", n, 4, "%d k=%d" % (n, k)):
-        L.check(lib.fqb200_kmeans1d(x.data_ptr(), n, num_bits, first, ptr(draws), kmeans_trials(k), ptr(init_t),
-                                    KMEANS_TASKS[task], rows, labels.data_ptr(), centres.data_ptr(), inertia.data_ptr(),
-                                    n_iter.data_ptr(), init_ids.data_ptr(), ptr(out), ptr(out_bcorr), ws.data_ptr(), need,
-                                    int(max_ctas), _stream_handle(dev)))
+    ws = _own_workspace(dev, lib.fqb200_kmeans1d_workspace_bytes(n, k))
+    _launch(dev, _Timed("C", n, 4, "%d k=%d" % (n, k)), lib.fqb200_kmeans1d, x.data_ptr(), n, num_bits, first, _ptr(draws),
+            kmeans_trials(k), _ptr(init_t), KMEANS_TASKS[task], rows, labels.data_ptr(), centres.data_ptr(),
+            inertia.data_ptr(), n_iter.data_ptr(), init_ids.data_ptr(), _ptr(out), _ptr(out_bcorr), ws.data_ptr(),
+            ws.numel(), int(max_ctas))
     return KMeans1d(labels, centres, inertia, n_iter, init_ids, out, out_bcorr)
 
 
@@ -676,8 +662,7 @@ def add_relu_(a, b):
     _require_cuda_f32(b, "b")
     if a.shape != b.shape or a.stride() != b.stride() or not dense(a):
         raise ValueError("add_relu_ needs two dense tensors of identical shape and strides")
-    with torch.cuda.device(a.device), _Timed("E", a.numel(), 12):
-        L.check(L.load().fqb200_add_relu(a.data_ptr(), b.data_ptr(), a.data_ptr(), a.numel(), _stream_handle(a.device)))
+    _launch(a.device, _Timed("E", a.numel(), 12), L.load().fqb200_add_relu, a.data_ptr(), b.data_ptr(), a.data_ptr(), a.numel())
     return a
 
 
@@ -701,9 +686,9 @@ def maxpool2d_cl(x, kernel_size, stride, padding, out=None):
     pitch = slice_pitch(user) if user is not None else 0
     direct = pitch >= c and pitch % 4 == 0 and user.data_ptr() % 16 == 0 and not _overlaps(x, user, pitch)
     kout = user if direct else torch.empty((n, c, oh, ow), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
-    with torch.cuda.device(x.device), _Timed("Pi" if direct and pitch != c else "P", kout.numel(), 4 + 4 * sh * sw):
-        L.check(L.load().fqb200_maxpool2d_nhwc_into(x.data_ptr(), kout.data_ptr(), n, h, w, c, kh, kw, sh, sw, ph, pw,
-                                                    pitch if direct else c, _stream_handle(x.device)))
+    _launch(x.device, _Timed("Pi" if direct and pitch != c else "P", kout.numel(), 4 + 4 * sh * sw),
+            L.load().fqb200_maxpool2d_nhwc_into, x.data_ptr(), kout.data_ptr(), n, h, w, c, kh, kw, sh, sw, ph, pw,
+            pitch if direct else c)
     return _finish_out(kout, None if direct else user)
 
 

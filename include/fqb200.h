@@ -210,7 +210,7 @@ int fqb200_quantize1(const float* in, float* out, float* grid, int64_t outer, in
  * first when relu_first, i.e. when a ReLU follows the convolution); out = y + q_bias where y > 0.  The tensor must be
  * channels-last ([outer][inner][groups] in memory, groups % 4 == 0, groups <= 2048).  Optional out_qbias receives the
  * `groups` corrections.  Workspace as for fqb200_fused (fqb200_workspace_bytes of any channels_last descriptor with the
- * same `groups`).  `out` may alias `in`.
+ * same `groups`, 16-byte aligned; FQB200_ERR_WORKSPACE otherwise, checked before any device call).  `out` may alias `in`.
  */
 int fqb200_quantize1_bca(const float* in, float* out, int64_t outer, int64_t groups, int64_t inner, const float* delta,
                          const float* offset, const float* bits, int per_group, int num_bits, const float* bias, int relu_first,

@@ -25,10 +25,17 @@ def _header_symbols():
     return sorted(set(re.findall(r"\b(fqb200_[a-z0-9_]+)\s*\(", src)))
 
 
+def _header_arities():
+    src = open(os.path.join(ROOT, "include", "fqb200.h")).read()
+    decls = re.findall(r"^(?:const )?\w+\*? ?(fqb200_[a-z0-9_]+)\(([^)]*)\);", src, re.M)
+    return {name: 0 if args.strip() == "void" else args.count(",") + 1 for name, args in decls}
+
+
 def test_library_exports_every_declared_symbol(lib):
     from cnn_quantization_b200 import _lib
     declared = _header_symbols()
     assert sorted(_lib.SYMBOLS) == declared
+    assert {name: len(argtypes) for name, (_, argtypes) in _lib.PROTOTYPES.items()} == _header_arities()
     out = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
     exported = set(line.split()[-1] for line in out.splitlines() if line.strip())
     for sym in declared:
@@ -70,13 +77,24 @@ def test_argument_validation_without_gpu(lib):
     assert lib.fqb200_float2gemmlowp(None, None, -1, 1.0, 0.0, 8, 0, 1, None, None) == _lib.ERR_INVALID
     assert lib.fqb200_float2gemmlowp(None, None, 0, 1.0, 0.0, 8, 0, 1, None, None) == _lib.OK  # empty tensor: no-op
     assert lib.fqb200_quantize1(None, None, None, 1, 4, 4, None, None, None, 1, 4, None, 0, None) == _lib.ERR_INVALID
-    # the plan query works without a device (it assumes an H100, 132 SMs): channels-last ResNet-50 layer, 3 phases on the
-    # bulk ring
+    # the plan query works without a device (it assumes an H100, 132 SMs, each kernel family at its __launch_bounds__
+    # residency): channels-last ResNet-50 layer, 3 phases on the bulk ring, one CTA per SM; RANGE_GIVEN takes twice as many
     d = _lib.Desc()
     d.outer, d.groups, d.inner, d.num_bits, d.range_mode, d.channels_last = 512, 256, 196, 4, _lib.RANGE_LAPLACE, 1
     out = (ctypes.c_int64 * 8)()
     assert lib.fqb200_plan_info(ctypes.byref(d), out) == _lib.OK
-    assert out[0] == 2 and 1 <= out[1] <= 264 and out[5] == 512 and out[7] == 3
+    assert out[0] == 2 and 1 <= out[1] <= 132 and out[5] == 512 and out[7] == 3
+    grid = out[1]
+    g = _lib.Desc()
+    g.outer, g.groups, g.inner, g.num_bits, g.range_mode, g.channels_last = 512, 256, 196, 4, _lib.RANGE_GIVEN, 1
+    g.given_delta = g.given_offset = 1 << 20
+    assert lib.fqb200_plan_info(ctypes.byref(g), out) == _lib.OK and out[1] == 2 * grid
+    # fqb200_quantize1_bca checks its workspace, size and 16-byte alignment, before any device call
+    need = lib.fqb200_workspace_bytes(ctypes.byref(d))
+    bca = (1 << 20, 1 << 20, 512, 256, 196, 1 << 20, 1 << 20, None, 1, 4, None, 0, None)
+    assert lib.fqb200_quantize1_bca(*bca, None, 0, None) == _lib.ERR_WORKSPACE
+    assert lib.fqb200_quantize1_bca(*bca, (1 << 20) + 4, need, None) == _lib.ERR_WORKSPACE
+    assert b"16-byte aligned" in lib.fqb200_last_error()
     d.groups = 96   # C/4 = 24 does not divide 512: 504 consumer threads take part
     assert lib.fqb200_plan_info(ctypes.byref(d), out) == _lib.OK and out[5] == 504
     d.groups = 6

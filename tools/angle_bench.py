@@ -15,37 +15,11 @@ Writing angle.pkl (once per run) is not measured.
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchlib import ROOT, build_or_exit, gpu_info, median, timed, write_json
 
 FP64_PEAK = 67e12   # H100 SXM data sheet, FP64 tensor core, FLOP/s
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
-
-
-def timed(fn):
-    import torch
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1)
-
-
-def median(v):
-    return sorted(v)[len(v) // 2]
 
 
 def main():
@@ -56,11 +30,8 @@ def main():
     ap.add_argument("--pairs", type=int, default=300, help="pairs of the reference's loop timed")
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_angle_bench.json"))
     a = ap.parse_args()
+    build_or_exit("angle_bench.py")
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("angle_bench.py measures on a CUDA device; none found")
-    import __graft_entry__
-    __graft_entry__.build()
     from cnn_quantization_b200 import ops, pipeline
     torch.backends.cudnn.benchmark = False
     torch.backends.cudnn.deterministic = True
@@ -81,7 +52,7 @@ def main():
         rates = {k: [] for k in arms}
         for _ in range(a.rounds):
             for k, (model, qm) in models.items():
-                t = timed(lambda: [model(xb) for _ in range(a.steps)])
+                t = timed(lambda: [model(xb) for _ in range(a.steps)])[0]
                 rates[k].append(a.batch * a.steps / (t * 1e-3))
                 if qm.measure_stats is not None:
                     qm.measure_stats.stats = {}   # keep only what one round measured
@@ -144,10 +115,7 @@ def main():
                 "to every pair of every measured tensor at that per-pair cost (not run end to end); angle.pkl is not "
                 "written or timed",
     }
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f)
-        f.write("\n")
+    write_json(res, a.out)
     print(json.dumps(res))
     s, r = res["sample_angles"], res["resnet50_w4a4_cl"]["images_per_s"]
     print("| `h100_angle_bench.json` | `python tools/angle_bench.py`: the angle kind of `-ms`. Taken on %s. ResNet-50 W4A4 "

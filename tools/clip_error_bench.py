@@ -12,41 +12,12 @@ Writing the summary files (once per run) is not measured.
 import argparse
 import json
 import os
-import subprocess
-import sys
 import tempfile
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchlib import ROOT, build_or_exit, gpu_info, median, timed, write_json
 
 HBM_PEAK = 3.35e12   # H100 SXM data sheet, bytes/s
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
-
-
-def timed(fn, reps):
-    import torch
-    ms = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return ms
-
-
-def median(v):
-    return sorted(v)[len(v) // 2]
 
 
 def main():
@@ -56,11 +27,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_clip_error_bench.json"))
     a = ap.parse_args()
+    build_or_exit("clip_error_bench.py")
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("clip_error_bench.py measures on a CUDA device; none found")
-    import __graft_entry__
-    __graft_entry__.build()
     from cnn_quantization_b200 import ops, pipeline
 
     # -- the kernel alone ------------------------------------------------------------------------------------------------
@@ -121,10 +89,7 @@ def main():
         "note": "hbm fraction against the 3.35 TB/s data sheet, 4 B/element; collect steps are host-clock times around a "
                 "synchronised forward (the collect path reads statistics back to the host per hooked tensor)",
     }
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f)
-        f.write("\n")
+    write_json(res, a.out)
     print(json.dumps(res))
     k, r = res["clip_error"], res["resnet50_collect_int4"]
     print("| `h100_clip_error_bench.json` | `python tools/clip_error_bench.py`: collect_err cost. Taken on %s. `ops.clip_error` "

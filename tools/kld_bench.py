@@ -14,12 +14,8 @@ it implies labelled as an extrapolation.
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchlib import build_or_exit, gpu_info, median, timed
 
 HBM_PEAK = 3.35e12               # H100 SXM data sheet, bytes/s
 REF_CPU_S_PER_SAMPLE = 0.33      # the reference's search per sample on a CPU host (measured, see the docstring)
@@ -39,25 +35,13 @@ def hooked_shapes(batch):
     return shapes
 
 
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=512)
     ap.add_argument("--reps", type=int, default=3)
     a = ap.parse_args()
+    build_or_exit("kld_bench.py")
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("kld_bench.py measures on a CUDA device; none found")
-    import __graft_entry__
-    __graft_entry__.build()
     from cnn_quantization_b200 import ops
 
     shapes = hooked_shapes(a.batch)
@@ -70,16 +54,7 @@ def main():
     for x in xs:   # warm-up: module load, shared-memory attributes
         ops.kld_threshold(x)
     torch.cuda.synchronize()
-    batch_ms = []
-    for _ in range(a.reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for x in xs:
-            th = ops.kld_threshold(x)[0]
-            th.max()
-        e1.record()
-        torch.cuda.synchronize()
-        batch_ms.append(e0.elapsed_time(e1))
+    batch_ms = timed(lambda: [ops.kld_threshold(x)[0].max() for x in xs], a.reps)
 
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -96,7 +71,7 @@ def main():
     res = {
         "tool": "kld_bench", "gpu": gpu_info(), "model": "resnet50", "batch": a.batch, "hooked_tensors": len(shapes),
         "rows": rows, "elements": elems,
-        "batch_ms_median": sorted(batch_ms)[len(batch_ms) // 2], "batch_ms_all": [round(v, 3) for v in batch_ms],
+        "batch_ms_median": median(batch_ms), "batch_ms_all": [round(v, 3) for v in batch_ms],
         "hist_phase_ms": round(hist_ms, 3), "absmax_ms": round(kern["absmax"], 3), "hist_ms": round(kern["hist"], 3),
         "hist_phase_gelem_s": round(elems / (hist_ms * 1e-3) / 1e9, 2) if hist_ms else None,
         "hist_phase_hbm_fraction": round(8.0 * elems / (hist_ms * 1e-3) / HBM_PEAK, 3) if hist_ms else None,

@@ -17,25 +17,13 @@ The input check of ops.kmeans1d (one host synchronisation) and the draws are out
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchlib import ROOT, build_or_exit, gpu_info, write_json
 
 HBM_PEAK = 3.35e12   # H100 SXM data sheet, bytes/s
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
 
 
 def timed(fn, reps):
@@ -58,10 +46,10 @@ def main():
     ap.add_argument("--sk", type=int, default=3)
     ap.add_argument("--configs", default="resnet50:4,resnet50:8,vgg16:4")
     a = ap.parse_args()
+    build_or_exit("kmeans_bench.py")
     import torch
     import cnn_quantization_b200 as fq
     from cnn_quantization_b200 import kmeans_quantization as KQ
-    assert torch.cuda.is_available(), "kmeans_bench needs a CUDA device"
     ops = fq.ops
     res = {"gpu": gpu_info(), "reps": a.reps, "configs": {}}
     for cfg in a.configs.split(","):
@@ -111,9 +99,7 @@ def main():
         res["configs"][cfg] = {"tensors": rows, "total": {k: (round(v, 3) if isinstance(v, float) else v) for k, v in tot.items()}}
         print(cfg, json.dumps(res["configs"][cfg]["total"]), flush=True)
         del model
-    os.makedirs(os.path.dirname(a.out), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f)
+    write_json(res, a.out)
     print(json.dumps(res)[:2000])
 
 

@@ -14,40 +14,11 @@ Writing distance.csv (once per run) is not measured.
 import argparse
 import json
 import os
-import subprocess
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchlib import ROOT, build_or_exit, gpu_info, median, timed, write_json
 
 HBM_PEAK = 3.35e12   # H100 SXM data sheet, bytes/s
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
-
-
-def timed(fn, reps):
-    import torch
-    ms = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return ms
-
-
-def median(v):
-    return sorted(v)[len(v) // 2]
 
 
 def main():
@@ -58,11 +29,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5, help="forwards per config per round")
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_measure_bench.json"))
     a = ap.parse_args()
+    build_or_exit("measure_bench.py")
     import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("measure_bench.py measures on a CUDA device; none found")
-    import __graft_entry__
-    __graft_entry__.build()
     from cnn_quantization_b200 import ops, pipeline
     torch.backends.cudnn.benchmark = False
     torch.backends.cudnn.deterministic = True
@@ -133,10 +101,7 @@ def main():
                 "'M' launches' event time of one profiled forward (derived, not timed on its own); the distance.csv write "
                 "is not measured",
     }
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f)
-        f.write("\n")
+    write_json(res, a.out)
     print(json.dumps(res))
     r = res["resnet50_w4a4_cl"]
     print("| `h100_measure_bench.json` | `python tools/measure_bench.py`: `-ms` cost. Taken on %s. `ops.sample_sumsq` on "

@@ -14,23 +14,10 @@ the forwards (images/s = batch * steps / time).  The logits of both arms on the 
 import argparse
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True, timeout=30).stdout.strip().splitlines()
-        return out[0] if out else "unknown"
-    except Exception:
-        return "unknown"
-
+from benchlib import ROOT, build_or_exit, gpu_info, timed, write_json
 
 OFF = {"inception_v3_w4a4": ("fuse_inception_concat", "skip_redundant_relu"), "vgg16_bn_w4a4": ("fuse_pool_into_quant",)}
 
@@ -55,11 +42,10 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--configs", default="inception_v3_w4a4,vgg16_bn_w4a4")
     a = ap.parse_args()
+    build_or_exit("paper_nets_bench.py")
     import torch
     from cnn_quantization_b200 import pipeline
-    if not torch.cuda.is_available():
-        raise SystemExit("no CUDA device: this tool measures on the GPU")
-    res = {"gpu": gpu_info(), "device": torch.cuda.get_device_name(), "batch": a.batch, "steps": a.steps,
+    res ={"gpu": gpu_info(), "device": torch.cuda.get_device_name(), "batch": a.batch, "steps": a.steps,
            "warmup": a.warmup, "rounds": a.rounds, "memory_format": "channels_last", "configs": {}}
     for config in a.configs.split(","):
         hw = pipeline.INPUT_SIZE[config]
@@ -76,13 +62,7 @@ def main():
             for r in range(a.rounds):
                 for name in (("fused", "unfused", "unfused", "fused") if r % 2 == 0 else ("unfused", "fused", "fused", "unfused")):
                     model = arms[name][0]
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    for _ in range(a.steps):
-                        model(x)
-                    e1.record()
-                    e1.synchronize()
-                    times[name].append(e0.elapsed_time(e1) / 1e3)
+                    times[name].append(timed(lambda: [model(x) for _ in range(a.steps)])[0] / 1e3)
         entry = {"hw": hw, "unfused_arm_disables": list(OFF[config]),
                  "logits_equal": bool(torch.equal(logits["fused"], logits["unfused"]))}
         for name, ts in times.items():
@@ -95,9 +75,7 @@ def main():
             qm.detach()
         del arms, x, logits
         torch.cuda.empty_cache()
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "w") as f:
-        json.dump(res, f)
+    write_json(res, a.out)
     print(json.dumps(res))
     if not all(e["logits_equal"] for e in res["configs"].values()):
         raise SystemExit("fused and unfused logits differ")
