@@ -1229,7 +1229,8 @@ __global__ void __launch_bounds__(kBulkThreads, kBulkCtasPerSm) fq_cl_bca_kernel
 // S1: min / max of every row (units never straddle rows; one CTA-wide combine + two atomics per unit), grid barrier, then
 // EVERY CTA derives the one parameter set itself from the <= 4096 row results (scope GROUP_MEAN: batch average of the
 // per-sample min / max, :372; scope TENSOR / one row: global min / max), A: apply.  The optional per-channel bias (folded
-// BN) is a per-thread constant on channels-last memory, where a vector's channels are (index mod C/4).
+// BN) is a per-thread constant on channels-last memory, where a vector's channels are (index mod C/4); with it the apply
+// phase can also write a channel slice of a wider channels-last tensor (FusedArgs::out_pad_v, fqb200_fused_into).
 struct RowsStats {
   const FusedArgs& A;
   float* scratch;  // [2][kWarps] floats in shared memory
@@ -1328,7 +1329,10 @@ struct RowsApply {
         y.w = y.w < 0.f ? 0.f : y.w;
       }
     }
-    st_tensor(reinterpret_cast<float4*>(A.out) + off, y);
+    // a channel slice of a wider channels-last tensor (out_pad_v, launches with a channel-fastest bias only): `off` counts
+    // cv = C/4 vectors per pixel, the output out_pad_v more
+    const unsigned o = A.out_pad_v ? off + (off / A.flat.cv) * A.out_pad_v : off;
+    st_tensor(reinterpret_cast<float4*>(A.out) + o, y);
   }
   __device__ __forceinline__ void consume(const float4& v, unsigned off) {
     if (dv.fast)

@@ -1829,17 +1829,30 @@ unsigned pool_tile_width(int kind, int64_t w, const fqb::FlatGeo& f) {
   return 0;
 }
 
+// The channel count C of a launch whose apply phase can write a channel slice of a wider channels-last tensor: a
+// channels-last launch's groups, or the period of the channel-fastest bias (bias_period = -C) of a per-sample / per-tensor
+// min-max launch, which reads channels-last memory as rows of samples and learns C from that bias as its in-launch pooling
+// does.  0: the launch cannot write a slice.
+int64_t slice_channels(const fqb200_desc* d) {
+  if (d->channels_last) return d->groups;
+  if (d->bias && d->bias_period < 0 && rows_supported(d, true)) return -d->bias_period;
+  return 0;
+}
+
 // What a pitched `out` (fqb200_fused_into, `pitch` floats between two pixels) needs beyond the descriptor's own route: the
-// apply phase of a channels-last launch without pooling / residual is the only store that can skip the other channels of a
-// pixel; a 16-byte aligned `out` (`can_vec`); and 32-bit vector offsets.  No CUDA calls: fqb200_fused_into checks it before
-// any device call, plan_fused again for the plan it makes.
+// apply phase of a launch with a slice_channels() C, without pooling / residual, is the only store that can skip the other
+// channels of a pixel; a 16-byte aligned `out` (`can_vec`); and 32-bit vector offsets.  No CUDA calls: fqb200_fused_into
+// checks it before any device call, plan_fused again for the plan it makes.
 int pitch_rules(const fqb200_desc* d, bool can_vec, int64_t pitch) {
-  if (!d->channels_last || d->stats_only || d->pool || d->residual)
-    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride: channels-last apply launches without pooling / residual only%s");
-  if (pitch < d->groups || pitch % 4 != 0)
+  const int64_t c = slice_channels(d);
+  if (!c || d->stats_only || d->pool || d->residual)
+    return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride: channels-last apply launches, or per-sample / per-tensor min-max apply "
+                                        "launches with a channel-fastest bias, without pooling / residual only%s");
+  if (pitch < c || pitch % 4 != 0)
     return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride must be >= C and a multiple of 4%s");
   if (!can_vec) return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride needs 16-byte aligned tensors%s");
-  const uint64_t pixels = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->inner);
+  const uint64_t pixels = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->groups) * static_cast<uint64_t>(d->inner) /
+                          static_cast<uint64_t>(c);
   if (pixels * static_cast<uint64_t>(pitch) / 4 >= (1ull << 32))
     return fail(FQB200_ERR_UNSUPPORTED, "out_pixel_stride: outputs of 2^32 vectors and more are not supported%s");
   return FQB200_OK;
@@ -1889,7 +1902,7 @@ int plan_fused(const fqb200_desc* d, bool can_vec, int64_t out_pitch, const Devi
   if (out_pitch) {
     rc = pitch_rules(d, can_vec, out_pitch);
     if (rc != FQB200_OK) return rc;
-    A.out_pad_v = static_cast<unsigned>((out_pitch - d->groups) / 4);
+    A.out_pad_v = static_cast<unsigned>((out_pitch - slice_channels(d)) / 4);
   }
   if ((d->residual_stats || d->residual_bias) && !d->residual)
     return fail(FQB200_ERR_INVALID, "residual_stats / residual_bias without a residual%s");
@@ -2216,22 +2229,25 @@ int fqb200_fused_into(const fqb200_desc* d, const float* in, float* out, int64_t
   if (!out && !d->stats_only && !d->pool) return fail(FQB200_ERR_INVALID, "null output%s");
   if (d->stats_only && !d->out_stats) return fail(FQB200_ERR_INVALID, "stats_only needs out_stats%s");
   const bool can_vec = aligned16(in) && (d->stats_only || d->pool || aligned16(out));
+  int64_t c = 0;   // channels of a pixel (slice_channels), when `out` is pitched
   if (out_pixel_stride != 0) {   // 0: fqb200_fused, a dense `out`
     if (out_pixel_stride < 0) return fail(FQB200_ERR_INVALID, "negative out_pixel_stride%s");
     rc = pitch_rules(d, can_vec, out_pixel_stride);
     if (rc != FQB200_OK) return rc;
-    const uint64_t pixels = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->inner);
-    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), i1 = i0 + pixels * d->groups * sizeof(float);
+    c = slice_channels(d);
+    const uint64_t elems = static_cast<uint64_t>(d->outer) * static_cast<uint64_t>(d->groups) * static_cast<uint64_t>(d->inner);
+    const uint64_t pixels = elems / static_cast<uint64_t>(c);
+    const uintptr_t i0 = reinterpret_cast<uintptr_t>(in), i1 = i0 + elems * sizeof(float);
     const uintptr_t o0 = reinterpret_cast<uintptr_t>(out),
-                    o1 = o0 + ((pixels - 1) * out_pixel_stride + d->groups) * sizeof(float);
-    if (out_pixel_stride != d->groups && o0 < i1 && i0 < o1)   // (the dense case may work in place)
+                    o1 = o0 + ((pixels - 1) * out_pixel_stride + c) * sizeof(float);
+    if (out_pixel_stride != c && o0 < i1 && i0 < o1)   // (the dense case may work in place)
       return fail(FQB200_ERR_INVALID, "out_pixel_stride: out overlaps in%s");
   }
   DeviceInfo* di = nullptr;
   rc = get_device(&di);
   if (rc != FQB200_OK) return rc;
   FusedPlan fp;
-  rc = plan_fused(d, can_vec, out_pixel_stride == d->groups ? 0 : out_pixel_stride, *di, &fp);   // pitch C: dense
+  rc = plan_fused(d, can_vec, out_pixel_stride == c ? 0 : out_pixel_stride, *di, &fp);   // pitch C: dense
   if (rc != FQB200_OK) return rc;
   rc = check_workspace(workspace, workspace_bytes, fp.workspace, "fqb200_workspace_bytes");
   if (rc != FQB200_OK) return rc;

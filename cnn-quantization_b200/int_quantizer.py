@@ -138,7 +138,8 @@ class IntQuantizer(object):
         ``bias``: a per-channel vector added to the tensor before anything else inside the kernel (the folded-BN
         convolution bias, so the convolution itself can run bias-free and a whole pass over the activation is saved);
         ``out``: a channel slice of a wider channels-last tensor (a branch's part of an Inception block's concatenation);
-        where the channels-last apply launch can write it (``ops.slice_eligible``) the result is written there and that
+        where the channels-last apply launch, or the per-sample / per-tensor min-max launch of a channels-last tensor with a
+        convolution bias, can write it (``ops.slice_eligible``) the result is written there and that
         slice comes back; otherwise the operand is ignored and the caller copies the result itself."""
         if override_att is not None:
             orig_att = getattr(self, override_att[0])
@@ -349,7 +350,9 @@ class IntQuantizer(object):
                 res._fq_pooled = pool[0]   # 2 / 3: which pooling the launch has done
                 return res
         rkw = self._residual_kw(tensor, channels_last, rows=rows, bias=kw.get("bias"))
-        if not rkw and self._into is not None and ops.slice_eligible(tensor, self._into, channels_last):
+        # (a rows launch knows C, and so the pixels of a slice, from its channel-fastest bias)
+        if not rkw and self._into is not None and ops.slice_eligible(tensor, self._into, channels_last,
+                                                                     bias_period=kw.get("bias_period", 0) if rows else 0):
             kw["out"] = self._into
         res = self._fused(tensor, layout, channels_last=channels_last, **kw, **rkw)
         if rkw:

@@ -154,12 +154,14 @@ def _overlaps(x, out, pitch):
     return o0 < x0 + 4 * x.numel() and x0 < o0 + 4 * ((pixels - 1) * pitch + out.shape[1])
 
 
-def slice_eligible(x, out, channels_last=True, stats_only=False, pool=None, residual=None):
+def slice_eligible(x, out, channels_last=True, stats_only=False, pool=None, residual=None, bias_period=0):
     """True when a launch of ``fused`` on ``x`` writes ``out``, a channel slice of a wider channels-last tensor
-    (``slice_pitch``), in place (C ABI fqb200_fused_into; the library applies the same rules): a channels-last apply launch
-    without pooling or residual on a ``cl_eligible`` x, the pixel pitch >= C and a multiple of 4, ``out`` 16-byte aligned,
-    not overlapping x."""
-    if (not channels_last or stats_only or pool is not None or residual is not None or not cl_eligible(x)
+    (``slice_pitch``), in place (C ABI fqb200_fused_into; the library applies the same rules): a channels-last apply launch,
+    or a per-sample / per-tensor min-max launch (``channels_last=False``) that knows C from its channel-fastest bias
+    (``bias_period`` = -C, at most 4096 samples), without pooling or residual on a ``cl_eligible`` x, the pixel pitch >= C
+    and a multiple of 4, ``out`` 16-byte aligned, not overlapping x."""
+    rows_cl = not channels_last and bias_period < 0 and -bias_period == x.shape[1] and x.shape[0] <= 4096
+    if (not (channels_last or rows_cl) or stats_only or pool is not None or residual is not None or not cl_eligible(x)
             or tuple(out.shape) != tuple(x.shape)):
         return False
     p = slice_pitch(out)
@@ -324,8 +326,9 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     """C ABI fqb200_fused: statistics -> parameters -> quantize/dequantize in one launch.
 
     Returns ``out`` (or ``(out, stats)`` with ``want_stats``; ``stats`` alone with ``stats_only``), where
-    ``stats`` is a [groups, 12] tensor with columns ``_lib.STAT_COLUMNS``.  A channels-last launch writes an ``out`` that is
-    a channel slice of a wider channels-last tensor directly (``slice_eligible``; profile mode suffix "i")."""
+    ``stats`` is a [groups, 12] tensor with columns ``_lib.STAT_COLUMNS``.  A channels-last launch, or a per-sample /
+    per-tensor min-max launch on channels-last memory with a channel-fastest bias (``bias_period`` = -C), writes an ``out``
+    that is a channel slice of a wider channels-last tensor directly (``slice_eligible``; profile mode suffix "i")."""
     _require_cuda_f32(x, "tensor")
     lib = L.load()
     is_cl = x.dim() == 4 and x.is_contiguous(memory_format=torch.channels_last)
@@ -439,7 +442,8 @@ def fused(x, layout, *, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.L
     pitch = 0
     if stats_only or pooled is not None:
         kout, uout = None, None
-    elif out is not None and out.stride() != x.stride() and slice_eligible(x, out, channels_last, residual=residual):
+    elif out is not None and out.stride() != x.stride() and slice_eligible(
+            x, out, channels_last, residual=residual, bias_period=bias_period if bias is not None and is_cl else 0):
         _require_cuda_f32(out, "out")
         kout, uout, pitch = out, None, slice_pitch(out)
     else:

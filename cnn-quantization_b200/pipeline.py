@@ -12,7 +12,8 @@ import torch.nn as nn
 
 from . import manager as M
 
-__all__ = ["CONFIGS", "INPUT_SIZE", "ARCH_KWARGS", "build_quantized_model", "synthetic_batch", "validate", "accuracy_counts", "reduce_metrics", "HostFeeder"]
+__all__ = ["CONFIGS", "INPUT_SIZE", "ARCH_KWARGS", "PAPER_NETS", "PAPER_TABLE", "paper_cell_input_size", "build_paper_cell",
+           "build_quantized_model", "synthetic_batch", "validate", "accuracy_counts", "reduce_metrics", "HostFeeder"]
 
 # BASELINE.json configs -> reference CLI flags
 _W4A4 = dict(qtype="int4", qweight="int4", clipping="laplace", per_channel_quant_weights=True, per_channel_quant_act=True,
@@ -34,6 +35,52 @@ INPUT_SIZE = {name: 299 if cfg["arch"] == "inception_v3" else 224 for name, cfg 
 # not loaded).  Inception-v3's auxiliary head only runs in training, but its two convolutions and its linear take ids in
 # construction order and its weights are quantized, which the reference's max_mse_order_id (conv0..conv95) presumes.
 ARCH_KWARGS = {"inception_v3": dict(aux_logits=True, transform_input=True, init_weights=False)}
+
+# The paper's results table (the reference's fig/experiments.png): six networks, three bit-width settings with their method
+# rows, and an FP32 column.  The paper gives no command lines; the cells read its section headings literally, with the
+# shared flags of the reference README's two commands:
+#
+#   setting  common flags                                              method -> added flags
+#   8W4A     qtype=int4, qweight=int8, per_channel_quant_act           baseline: none; aciq: clipping=laplace;
+#                                                                      bit_alloc: bit_alloc_act;
+#                                                                      aciq_bit_alloc: clipping=laplace, bit_alloc_act
+#   4W8A     qtype=int8, qweight=int4, per_channel_quant_weights       baseline: none; bias_corr: bias_corr_weight;
+#                                                                      bit_alloc: bit_alloc_weight;
+#                                                                      bias_corr_bit_alloc: bit_alloc_weight, bias_corr_weight
+#   4W4A     qtype=int4, qweight=int4, per_channel_quant_weights,      baseline: none; all: clipping=laplace, bit_alloc_act,
+#            per_channel_quant_act                                     bit_alloc_weight, bias_corr_weight
+#   FP32     q_off=True                                                fp32: one cell per network
+#
+# 6 x (4 + 4 + 2 + 1) = 66 cells, keyed (net, setting, method) with the torchvision arch name as net; each value is the
+# ``make_args`` keywords of the cell, arch included.  Every cell uses the default bit-allocation target (the bit width).
+# So the "4W4A all" cell equals ``CONFIGS["<net>_w4a4"]`` for resnet18/50/101, inception_v3 and vgg16_bn, but not for
+# vgg16: ``vgg16_w4a4`` is BASELINE's bin-allocation run at a 5.3-bit target, not the paper's cell.
+PAPER_NETS = ("vgg16", "vgg16_bn", "inception_v3", "resnet18", "resnet50", "resnet101")
+_PAPER_SETTINGS = {
+    "8W4A": (dict(qtype="int4", qweight="int8", per_channel_quant_act=True), {
+        "baseline": {}, "aciq": dict(clipping="laplace"), "bit_alloc": dict(bit_alloc_act=True),
+        "aciq_bit_alloc": dict(clipping="laplace", bit_alloc_act=True)}),
+    "4W8A": (dict(qtype="int8", qweight="int4", per_channel_quant_weights=True), {
+        "baseline": {}, "bias_corr": dict(bias_corr_weight=True), "bit_alloc": dict(bit_alloc_weight=True),
+        "bias_corr_bit_alloc": dict(bit_alloc_weight=True, bias_corr_weight=True)}),
+    "4W4A": (dict(qtype="int4", qweight="int4", per_channel_quant_weights=True, per_channel_quant_act=True), {
+        "baseline": {}, "all": dict(clipping="laplace", bit_alloc_act=True, bit_alloc_weight=True, bias_corr_weight=True)}),
+    "FP32": (dict(q_off=True), {"fp32": {}}),
+}
+PAPER_TABLE = {(net, setting, method): dict(arch=net, **common, **added)
+               for net in PAPER_NETS for setting, (common, methods) in _PAPER_SETTINGS.items()
+               for method, added in methods.items()}
+
+
+def paper_cell_input_size(cell):
+    """The square crop of a PAPER_TABLE cell, ``(net, setting, method)``: 299 for Inception-v3, 224 otherwise."""
+    return 299 if cell[0] == "inception_v3" else 224
+
+
+def build_paper_cell(cell, device, seed=12345, quantizer_factory=None, channels_last=False):
+    """``build_quantized_model`` for a PAPER_TABLE cell, ``(net, setting, method)``: (model, manager)."""
+    return build_quantized_model(PAPER_TABLE[tuple(cell)], device, seed=seed, quantizer_factory=quantizer_factory,
+                                 channels_last=channels_last)
 
 
 def build_quantized_model(config, device, seed=12345, quantizer_factory=None, channels_last=False):
@@ -60,7 +107,8 @@ def build_quantized_model(config, device, seed=12345, quantizer_factory=None, ch
     model.to(device)
     if channels_last:
         model.to(memory_format=torch.channels_last)
-    qm.quantize_model(model)
+    if qm.quantize:   # without a qtype (the FP32 column: q_off alone) there are no weight quantizers; the weights stay fp32
+        qm.quantize_model(model)
     qm.attach(model)
     return model, qm
 

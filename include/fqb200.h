@@ -249,12 +249,17 @@ int fqb200_fused(const fqb200_desc* d, const float* in, float* out, void* worksp
                  void* stream);
 /*
  * fqb200_fused writing its result into a channel slice of a wider channels-last tensor
- * [outer][inner][out_pixel_stride]: pixel p of the result goes to out + p * out_pixel_stride (out points at the slice's
+ * [pixels][out_pixel_stride]: pixel p of the result goes to out + p * out_pixel_stride (out points at the slice's
  * first channel); the other channels of every pixel are left untouched.  A branch of an Inception block writes its part
  * of the concatenation this way, bit for bit what fqb200_fused followed by a copy would give.
- * Channels-last apply launches only (on-the-fly statistics, RANGE_GIVEN, torch and mid-tread leaves).
- * FQB200_ERR_UNSUPPORTED: stats_only, pool, residual or a non-channels-last descriptor; out_pixel_stride < groups or not
- * a multiple of 4; a misaligned in / out.  out_pixel_stride = groups is the dense case, where `out` may alias `in`; with
+ * Two kinds of apply launch take a pitch, C being the channels of a pixel:
+ *   - channels-last launches (on-the-fly statistics, RANGE_GIVEN, torch and mid-tread leaves): C = groups, pixels =
+ *     outer * inner;
+ *   - per-sample / per-tensor min-max launches (compiled leaf, outer = 1, groups = samples) on channels-last memory with a
+ *     channel-fastest bias: C = -bias_period, element (n, pixel, c) goes to out + (n * H*W + pixel) * out_pixel_stride + c.
+ *     Without such a bias the launch does not know C and takes no pitch.
+ * FQB200_ERR_UNSUPPORTED: stats_only, pool, residual, out_hist or any other descriptor; out_pixel_stride < C or not
+ * a multiple of 4; a misaligned in / out.  out_pixel_stride = C is the dense case, where `out` may alias `in`; with
  * any other pitch an `out` overlapping `in` returns FQB200_ERR_INVALID.  These rules are checked before any device call.
  * fqb200_fused(d, ...) is fqb200_fused_into(d, ..., 0, ...): a dense `out` for any descriptor.
  */
