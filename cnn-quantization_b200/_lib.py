@@ -76,6 +76,8 @@ PROTOTYPES = {
     "fqb200_kmeans1d_workspace_bytes": (_sz, [_i64, _i32]),
     "fqb200_sample_angles": (_i32, [_vp, _i64, _i64, _vp, _vp, _vp, _sz, _i32, _vp]),
     "fqb200_sample_angles_workspace_bytes": (_sz, [_i64, _i64]),
+    "fqb200_sample_noise": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _sz, _i32, _vp]),
+    "fqb200_sample_noise_workspace_bytes": (_sz, [_i64, _i64]),
 }
 SYMBOLS = tuple(PROTOTYPES)
 

@@ -1105,6 +1105,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_cliperr.cuh"
 #include "fq_kmeans.cuh"
 #include "fq_angle.cuh"
+#include "fq_noise.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1693,6 +1694,30 @@ size_t sumsq_workspace(int64_t rows, int64_t row_len) {
 size_t angle_workspace(int64_t rows, int64_t row_len) {
   const fqb::AngleSplit s = fqb::angle_split(static_cast<unsigned long long>(rows), static_cast<unsigned long long>(row_len));
   return static_cast<size_t>(s.pairs * s.slices) * fqb::kAngTile * fqb::kAngTile * 8;
+}
+
+// quantization-noise workspace: kNoiseSums float64 partials per (row, chunk) unit when a row spans several chunks
+// (fq_noise.cuh; enough for the two sums of a call without q too)
+size_t noise_workspace(int64_t rows, int64_t row_len) {
+  const unsigned long long chunk = fqb::noise_chunk(static_cast<unsigned long long>(row_len));
+  const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
+  return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * fqb::kNoiseSums * 8 : 0;
+}
+
+// fq_noise_partial_kernel for a bias mode and with or without q
+template <int VEC>
+void launch_noise(int mode, bool q, int grid, cudaStream_t st, const fqb::NoiseArgs& A) {
+  using namespace fqb;
+  if (mode == kNoiseBiasNchw) {
+    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasNchw><<<grid, kNoiseThreads, 0, st>>>(A);
+    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasNchw><<<grid, kNoiseThreads, 0, st>>>(A);
+  } else if (mode == kNoiseBiasCl) {
+    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasCl><<<grid, kNoiseThreads, 0, st>>>(A);
+    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasCl><<<grid, kNoiseThreads, 0, st>>>(A);
+  } else {
+    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasNone><<<grid, kNoiseThreads, 0, st>>>(A);
+    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasNone><<<grid, kNoiseThreads, 0, st>>>(A);
+  }
 }
 
 // clipping-error workspace: kCeSums float64 partials per (group, unit) (fq_cliperr.cuh)
@@ -2503,6 +2528,58 @@ int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* 
   const dim3 fgrid(fqb::kAngTile * fqb::kAngTile / fqb::kAngFinishThreads, static_cast<unsigned>(A.pairs));
   fqb::fq_gram_finish_kernel<<<fgrid, fqb::kAngFinishThreads, 0, st>>>(A);
   return launched("Gram kernels");
+}
+
+size_t fqb200_sample_noise_workspace_bytes(int64_t rows, int64_t row_len) {
+  g_err[0] = 0;
+  if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s"), 0;
+  return noise_workspace(rows, row_len);
+}
+
+int fqb200_sample_noise(const float* y, const float* q, const float* bias, int64_t bias_period, int64_t rows, int64_t row_len,
+                        double* out, void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s");
+  if (!y || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  const unsigned long long period = bias_period < 0 ? 0ull - static_cast<unsigned long long>(bias_period)
+                                                    : static_cast<unsigned long long>(bias_period);
+  if (bias) {
+    if (period == 0 || static_cast<unsigned long long>(row_len) % period != 0)
+      return fail(FQB200_ERR_INVALID, "a bias needs a bias_period != 0 whose magnitude divides row_len%s");
+    if (static_cast<unsigned long long>(row_len) > 0xffffffffull)
+      return fail(FQB200_ERR_UNSUPPORTED, "rows of 2^32 elements and more take no bias%s");
+  }
+  int rc = check_workspace(workspace, workspace_bytes, noise_workspace(rows, row_len), "fqb200_sample_noise_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  if (rows == 0) return FQB200_OK;
+  DeviceInfo* di = nullptr;
+  rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::NoiseArgs A;
+  memset(&A, 0, sizeof(A));
+  A.y = y;
+  A.q = q;
+  A.bias = bias;
+  A.period = static_cast<unsigned>(period);
+  A.rows = static_cast<unsigned long long>(rows);
+  A.row_len = static_cast<unsigned long long>(row_len);
+  A.chunk = fqb::noise_chunk(A.row_len);
+  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
+  A.sums = q ? fqb::kNoiseSums : 2;
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  const int grid = grid_for(A.rows * A.chunks, di->sms * (2048ull / fqb::kNoiseThreads), max_ctas);
+  const bool vec = row_len % 4 == 0 && aligned16(y) && (!q || aligned16(q));
+  const int mode = !bias ? fqb::kNoiseBiasNone : bias_period > 0 ? fqb::kNoiseBiasNchw : fqb::kNoiseBiasCl;
+  if (vec) launch_noise<4>(mode, q != nullptr, grid, st, A);
+  else     launch_noise<1>(mode, q != nullptr, grid, st, A);
+  if (A.chunks > 1) {
+    const unsigned long long blocks = (A.rows * A.sums + fqb::kNoiseThreads - 1) / fqb::kNoiseThreads;
+    fqb::fq_noise_finish_kernel<<<static_cast<unsigned>(blocks), fqb::kNoiseThreads, 0, st>>>(A);
+  }
+  return launched("quantization-noise kernels");
 }
 
 // the layouts fqb200_clip_error takes (argument errors as a message, nullptr when they are fine)

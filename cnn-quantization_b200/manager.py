@@ -33,8 +33,9 @@ def make_args(**over):
     """An ``args`` namespace with the reference CLI's defaults (inference/inference_sim.py:52-112) for the fields the
     manager and the quantizers read.  Extensions without a reference flag: ``stats_base_dir``, ``collect_err`` (fill the
     mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument) and
-    ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms, or "angle", the
-    pairwise sample angles of its angle_stats module, which the reference selects by editing an import)."""
+    ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms; "angle", the
+    pairwise sample angles of its angle_stats module, which the reference selects by editing an import; or "noise", the
+    per-sample quantization error statistics of its measure_statistics module, which the reference cannot run)."""
     d = dict(arch="resnet18", qtype=None, qweight="int8", q_off=False, clipping="no", stats_mode="no", stats_kind="mean",
              stats_folder=None, stats_batch_avg=False, kld_threshold=False, measure_stats=False,
              per_channel_quant_weights=False, per_channel_quant_act=False, bit_alloc_act=False, bit_alloc_weight=False,
@@ -378,19 +379,25 @@ class QuantizationManagerInference(object):
         # non-absorbed BN call site hands on.  Three launches never write that tensor - the block epilogue writes
         # max(q + identity, 0), a deferred shortcut is quantized only inside the consuming launch, a pooling launch writes
         # the pooled quarter - so they are switched off; each is bit-identical to its unfused form.
+        # The noise kind also measures the tensor the quantizer was handed, so activations are quantized out of place and
+        # that tensor survives the launch; the convolution bias stays fused and is passed to the measurement.
         self.measure_stats = None
         kind = getattr(args, "measure_stats_kind", "distance")
-        if kind not in ("distance", "angle"):
-            raise ValueError("measure_stats_kind must be 'distance' or 'angle', got %r" % (kind,))
+        if kind not in ("distance", "angle", "noise"):
+            raise ValueError("measure_stats_kind must be 'distance', 'angle' or 'noise', got %r" % (kind,))
         if args.measure_stats:
+            if kind == "noise" and self.stats_mode == "collect":
+                raise ValueError("measure_stats_kind='noise' measures quantization noise: collect mode quantizes nothing")
             import torch.distributed as dist
             if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
                 raise NotImplementedError("-ms with several ranks: per-rank shards would put the rows out of sample order")
-            from .statistics import AngleStatistics, MeasureStatistics
-            cls = AngleStatistics if kind == "angle" else MeasureStatistics
+            from .statistics import AngleStatistics, MeasureStatistics, NoiseStatistics
+            cls = {"distance": MeasureStatistics, "angle": AngleStatistics, "noise": NoiseStatistics}[kind]
             self.measure_stats = cls(args.arch, getattr(args, "stats_base_dir", None))
             self.fuse_residual_into_quant = self.defer_shortcut = self.fuse_pool_into_quant = False
             self.fuse_inception_concat = False   # the hooked output is the tensor -ms measures; keep torch.cat's
+            if kind == "noise":
+                self.inplace_activations = False
         # `collect_err`: the collect hooks hand each tensor's use-mode quantizer settings to save_tensor_stats, which fills
         # the mse_* / cos_* columns `-c mix` chooses by
         self.collect_err = bool(getattr(args, "collect_err", False))
@@ -537,7 +544,7 @@ class QuantizationManagerInference(object):
         if self.stats_manager is not None:
             self.stats_manager.__exit__()  # collect mode: write the CSV / pickle files
         if self.measure_stats is not None:
-            self.measure_stats.__exit__()  # -ms: write distance.csv (angle.pkl with the angle kind)
+            self.measure_stats.__exit__()  # -ms: write distance.csv (angle.pkl, noise/<id>.csv with the other kinds)
 
     # -- call sites: forward hooks reproducing the *WithId.forward bodies (:58-74, :84-101, :162-217, :227-250, :262-283)
     def attach(self, model):
@@ -648,11 +655,23 @@ class QuantizationManagerInference(object):
     def _measuring(self, hook, id_format):
         """``hook`` followed by the `-ms` measurement of what the call site hands on: the hook's result, or ``out`` where
         the hook leaves it (collect mode, quantization disabled).  Measured whether or not quantization is enabled, as the
-        reference's *WithId modules do; an absorbed BN (the identity) is not a measured site."""
+        reference's *WithId modules do; an absorbed BN (the identity) is not a measured site.  The noise kind measures
+        that tensor against ``out`` (plus the convolution bias the launch added to it), with ``inputs[0]`` and the
+        module's weight (a BN's gamma)."""
+        from . import ops
+        from .statistics import NoiseStatistics
+        noise = isinstance(self.measure_stats, NoiseStatistics)
+
         def measured(m, inputs, out):
             res = hook(m, inputs, out)
             if not (isinstance(m, nn.BatchNorm2d) and self.bn_folding and hasattr(m, "absorbed")):
-                self.measure_stats.save_measure(out if res is None else res, id_format % m._fq_id)
+                handed_on, id = out if res is None else res, id_format % m._fq_id
+                if noise:
+                    bias = getattr(m, "_fq_bias", None)   # a fused convolution bias: out is bias-free
+                    period = 0 if bias is None else (-out.shape[1] if ops.nhwc(out) else out[0, 0].numel())
+                    self.measure_stats.save_measure(out, handed_on, inputs[0], m.weight, id, bias=bias, bias_period=period)
+                else:
+                    self.measure_stats.save_measure(handed_on, id)
             return res
 
         return measured

@@ -24,8 +24,9 @@ def profile_collect():
     """Synchronise and return {'launches': n, 'modes': {mode: {launches, elems, bytes, ms}}}.  Modes by algorithmic
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
-    (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'E' the clipping-error measurement
-    (ops.clip_error) and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing."""
+    (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'N' the quantization-noise measurement
+    (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error) and 'C' the k-means clustering of a weight
+    tensor (ops.kmeans1d), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -538,6 +539,45 @@ def sample_angles(x, return_gram=False, max_ctas=0):
         _launch(dev, _Timed("G", x.numel(), 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_angles, x.data_ptr(), rows,
                 row_len, angles.data_ptr(), _ptr(gram), _ptr(ws), need, int(max_ctas))
     return (angles, gram) if return_gram else angles
+
+
+NOISE_SUMS = ("y", "y2", "q", "q2", "yq", "e", "e2")
+
+
+def sample_noise(y, q=None, bias=None, bias_period=0, max_ctas=0):
+    """C ABI fqb200_sample_noise: per sample (dim 0) of ``y`` the float64 sums behind the quantization-noise measurement
+    (measure_statistics.py:19-99) as a float64 [N, 7] device tensor, columns ``NOISE_SUMS``: sum y, y^2, q, q^2, y*q, e, e^2
+    with e = y - q in float64; without ``q`` the [N, 2] sums of y and y^2 (a layer input; a weight as one row).  ``q`` has
+    y's shape (read in y's memory order; copied when its strides differ).  ``bias`` (float32 [C]) is added to y first, as
+    the single fp32 add of a quantization launch with a convolution bias: ``bias_period`` H*W for an NCHW ``y``, -C for a
+    channels-last one.  Deterministic (the bits depend neither on the run nor on ``max_ctas``), no host synchronisation.
+    Recorded in the launch profile under mode 'N' (one read of y and q: 8 B/element, 4 without q)."""
+    y, rows, row_len = _samples(y, "sample_noise")
+    dev = y.device
+    if q is not None:
+        _require_cuda_f32(q, "q")
+        if q.shape != y.shape:
+            raise ValueError("sample_noise: q has shape %s, y %s" % (tuple(q.shape), tuple(y.shape)))
+        if q.stride() != y.stride():
+            q = torch.empty_like(y).copy_(q)   # y's dense memory order
+    if bias is not None:
+        _require_cuda_f32(bias, "bias")
+        bias = bias.contiguous()
+        c, period = bias.numel(), int(bias_period)
+        if not ((period > 0 and c * period == row_len) or (period < 0 and c == -period and row_len % c == 0)):
+            raise ValueError("sample_noise: a bias of %d values on rows of %d elements needs bias_period %d (NCHW) or "
+                             "%d (channels-last), got %d" % (c, row_len, row_len // max(c, 1), -c, period))
+    shape = (rows, len(NOISE_SUMS) if q is not None else 2)
+    if rows == 0 or y.numel() == 0:
+        return torch.zeros(shape, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
+    out = torch.empty(shape, dtype=torch.float64, device=dev)
+    lib = L.load()
+    need = lib.fqb200_sample_noise_workspace_bytes(rows, row_len)
+    ws = _own_workspace(dev, need, required=False)
+    _launch(dev, _Timed("N", y.numel(), 8 if q is not None else 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_noise,
+            y.data_ptr(), _ptr(q), _ptr(bias), int(bias_period), rows, row_len, out.data_ptr(), _ptr(ws), need,
+            int(max_ctas))
+    return out
 
 
 CLIP_ERROR_CANDIDATES = ("lowp", "gaus", "laplace")

@@ -32,6 +32,14 @@ Each hooked tensor costs one ops.sample_sumsq launch; the results stay on the de
 
 Each hooked tensor costs one ops.sample_angles launch pair; the float32 [N, N] matrices stay on the device until
 ``__exit__`` (1 MB per measured tensor and batch at N = 512: about 54 MB per ResNet-50 batch).
+
+``NoiseStatistics`` is the quantization-noise measurement (measure_statistics.py:19-99): the error each call site's
+quantizer put into its output, with the moments of the layer's input, output and weight:
+
+    <base>/noise/<folder>/<id>.csv       columns NOISE_COLUMNS, one row per sample in call order
+
+Each hooked tensor costs two ops.sample_noise launch pairs (output with its quantized form, input) and each weight one,
+once; the float64 sums stay on the device until ``__exit__`` (72 B per sample and call).
 """
 import collections
 import os
@@ -44,8 +52,8 @@ import torch
 
 from . import ops
 
-__all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "AngleStatistics", "ClipErrConfig",
-           "default_base_dir"]
+__all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "AngleStatistics", "NoiseStatistics",
+           "ClipErrConfig", "default_base_dir"]
 
 
 def default_base_dir():
@@ -407,3 +415,118 @@ class AngleStatistics(object):
         with open(os.path.join(self.folder, "angle.pkl"), "wb") as f:
             pickle.dump(out, f)
         self.stats = {}
+
+
+NOISE_COLUMNS = ["eps_norm", "eps_mse", "eps_cos_sim", "eps_ang_dist", "eps_mean", "eps_var", "w_mean", "w_var", "w_norm",
+                 "w_size", "x_mean", "x_var", "x_norm", "x_size", "y_mean", "y_var", "y_norm", "y_size", "c_out"]
+
+
+def _memory_rows(t, like):
+    """[N, row_len] of ``t``'s samples in the memory order of ``like``'s (channels-last rows as stored)."""
+    if ops.nhwc(like):
+        t = t.permute(0, 2, 3, 1)
+    return t.reshape(t.shape[0], -1)
+
+
+def sample_noise_cpu(y, q=None, bias=None, bias_period=0):
+    """ops.sample_noise for CPU tensors: the same float64 sums (columns ops.NOISE_SUMS, the first two without ``q``), with
+    ``bias`` added to y in fp32 by the same row convention."""
+    yr = _memory_rows(y, y)
+    if bias is not None:
+        i = torch.arange(yr.shape[1])
+        yr = yr + bias.float()[i // bias_period if bias_period > 0 else i % -bias_period]
+    yd = yr.double()
+    cols = [yd.sum(1), (yd * yd).sum(1)]
+    if q is not None:
+        qd = _memory_rows(q, y).double()
+        e = yd - qd
+        cols += [qd.sum(1), (qd * qd).sum(1), (yd * qd).sum(1), e.sum(1), (e * e).sum(1)]
+    return torch.stack(cols, 1)
+
+
+def noise_columns(yq, xs, ws, y_size, x_size, w_size, c_out):
+    """The NOISE_COLUMNS of measure_statistics.py:19-99 (float64 [rows, 19], rounded once to float32) from float64 sums:
+    ``yq`` [rows, 7] (ops.NOISE_SUMS of the output and its quantized form), ``xs`` / ``ws`` [rows, 2] (sum, sum of squares
+    of the input / the weight; NaN without a weight) and the per-row sizes.  Variances are population variances,
+    E[t^2] - E[t]^2 in float64 (at least 0).  The cosine is clamped to [-1, 1] before arccos; a zero sample gives a NaN
+    cosine and an angular distance of 0, as nan_to_num does in the reference."""
+    def mean_var_norm(s, s2, n):
+        m = s / n
+        return m, np.maximum(s2 / n - m * m, 0.0), np.sqrt(s2)
+
+    rows = yq.shape[0]
+    y_size, x_size, w_size, c_out = (np.broadcast_to(np.asarray(v, dtype=np.float64), (rows,))
+                                     for v in (y_size, x_size, w_size, c_out))
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        cos = yq[:, 4] / np.sqrt(yq[:, 1] * yq[:, 3])
+        e_mean, e_var, e_norm = mean_var_norm(yq[:, 5], yq[:, 6], y_size)
+        cols = [e_norm, yq[:, 6] / y_size, cos, np.nan_to_num(np.arccos(np.clip(cos, -1.0, 1.0))) / np.pi, e_mean, e_var]
+        w_mean, w_var, w_norm = mean_var_norm(ws[:, 0], ws[:, 1], w_size)
+        cols += [w_mean, w_var, w_norm, w_size]
+        x_mean, x_var, x_norm = mean_var_norm(xs[:, 0], xs[:, 1], x_size)
+        cols += [x_mean, x_var, x_norm, x_size]
+        y_mean, y_var, y_norm = mean_var_norm(yq[:, 0], yq[:, 1], y_size)
+        cols += [y_mean, y_var, y_norm, y_size, c_out]
+    return np.stack(cols, 1).astype(np.float32).astype(np.float64)
+
+
+class NoiseStatistics(object):
+    """Quantization noise of every measured call site (measure_statistics.py:19-99): ``save_measure(y, y_with_noise, x, w,
+    id)`` records, per sample, the error eps = y - y_with_noise (norm, MSE, cosine and angular distance between y and
+    y_with_noise, mean, variance) and the mean, variance, norm and size of the input x, the output y and the weight w,
+    plus c_out = w.shape[0]; ``__exit__`` writes one CSV per id, columns NOISE_COLUMNS, one row per sample in call order.
+    ``bias`` / ``bias_period`` (ops.sample_noise): a convolution bias the quantization launch added to y itself.  ``w``
+    None (a BN without affine parameters): the w_* columns are NaN and c_out is y's channel count.  The weight's moments
+    are computed on an id's first call and reused.
+
+    The reference leaves the output location unset (its module is never wired up); <base>/noise/<folder>/ beside
+    distance/ and angle/ is this project's choice.  Differences from the reference: everything is computed in float64 and
+    rounded once to float32 (the reference computes in fp32), and the cosine is clamped to [-1, 1] before arccos, where the
+    reference's fp32 cosine can step over 1 and give NaN, which its nan_to_num turns into the same 0."""
+
+    def __init__(self, folder, base_dir=None):
+        self.folder = os.path.join(base_dir or default_base_dir(), "noise", folder)
+        self.stats = {}     # id -> [(yq sums [N, 7], x sums [N, 2], y_size, x_size)], one per call
+        self.weights = {}   # id -> (weight sums [1, 2] or None, w_size, c_out)
+
+    def save_measure(self, y, y_with_noise, x, w, id, bias=None, bias_period=0):
+        y, q, x = y.detach(), y_with_noise.detach(), x.detach()
+        # enqueued now: later in-place writes to these tensors come after the launches in stream order
+        f = ops.sample_noise if y.is_cuda else sample_noise_cpu
+        yq = f(y, q, bias, bias_period)
+        xs = f(x)
+        if id not in self.weights:
+            if w is None:
+                self.weights[id] = (None, float("nan"), y.shape[1])
+            else:
+                w = w.detach()
+                self.weights[id] = (f(w.reshape(1, -1)), w.numel(), w.shape[0])
+        self.stats.setdefault(id, []).append((yq, xs, y[0].numel(), x[0].numel()))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *args):
+        if not self.stats:
+            return
+        import pandas as pd
+        tables = {}
+        for id, calls in self.stats.items():
+            wsum, w_size, c_out = self.weights[id]
+            parts = [c[0].reshape(-1) for c in calls] + [c[1].reshape(-1) for c in calls]
+            if wsum is not None:
+                parts.append(wsum.reshape(-1).to(parts[0].device))
+            flat = torch.cat(parts).cpu().numpy()   # one device-to-host copy per id
+            rows = sum(c[0].shape[0] for c in calls)
+            yq = flat[:rows * 7].reshape(rows, 7)
+            xs = flat[rows * 7:rows * 9].reshape(rows, 2)
+            ws = np.tile(flat[rows * 9:] if wsum is not None else np.full(2, np.nan), (rows, 1))
+            n = [c[0].shape[0] for c in calls]
+            tables[id] = noise_columns(yq, xs, ws, np.repeat([c[2] for c in calls], n), np.repeat([c[3] for c in calls], n),
+                                       w_size, c_out)
+        if os.path.exists(self.folder):
+            shutil.rmtree(self.folder)
+        os.makedirs(self.folder)
+        for id, table in tables.items():
+            pd.DataFrame(columns=NOISE_COLUMNS, data=table).to_csv(os.path.join(self.folder, "%s.csv" % id), index=False)
+        self.stats, self.weights = {}, {}

@@ -322,6 +322,30 @@ int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* 
 size_t fqb200_sample_angles_workspace_bytes(int64_t rows, int64_t row_len);
 
 /*
+ * Quantization-noise measurement (measure_statistics.py:19-99): for `rows` contiguous rows of `row_len` floats (one
+ * sample; any dense memory order of it, the same for y and q), the float64 sums of y and of its quantized form q:
+ *   q != NULL: out[r * 7 + k], k = 0 sum y, 1 sum y^2, 2 sum q, 3 sum q^2, 4 sum y*q, 5 sum e, 6 sum e^2 with e = y - q
+ *              formed in float64;
+ *   q == NULL: out[r * 2 + k], k = 0 sum y, 1 sum y^2 (the layer input, or a weight as one row).
+ * `bias` (optional) is added to y first, as the single fp32 add of a quantization launch with fqb200_desc.bias, in its
+ * row convention: bias_period > 0 gives element i of a row bias[i / bias_period] (NCHW, bias_period = H*W), < 0
+ * bias[i % -bias_period] (channels-last, -C); |bias_period| must divide row_len, and rows with a bias hold fewer than 2^32
+ * elements (FQB200_ERR_UNSUPPORTED).  bias_period is ignored without a bias.  Work units are (row, chunk) with a chunk
+ * length that depends on row_len only; each unit's partials go to the workspace and a row's partials are added in chunk
+ * order, so the bits do not depend on the run or on max_ctas (0: the default grid, else at most that many CTAs).  One
+ * read of y and q (16-byte loads where rows are 16-byte aligned, scalar loads otherwise) plus, when a row spans several
+ * chunks, a small second launch, on `stream`; no host synchronisation.  NaN and Inf propagate; rows == 0 launches nothing.
+ * The workspace (fqb200_sample_noise_workspace_bytes, 16-byte aligned; may be null when that is 0) is private to the call.
+ * FQB200_ERR_INVALID: rows < 0, row_len <= 0, max_ctas < 0, y or out null, a bias with a bias_period that does not fit;
+ * FQB200_ERR_WORKSPACE: a workspace that is missing, too small or misaligned.
+ */
+int fqb200_sample_noise(const float* y, const float* q, const float* bias, int64_t bias_period, int64_t rows, int64_t row_len,
+                        double* out, void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream);
+/* Workspace of fqb200_sample_noise in bytes, with or without q (0 and fqb200_last_error() on bad arguments: rows < 0,
+ * row_len <= 0). */
+size_t fqb200_sample_noise_workspace_bytes(int64_t rows, int64_t row_len);
+
+/*
  * Clipping-error measurement (the mse_* / cos_* columns of `-sm collect`, statistic_manager.py:83-111): for every group g
  * of x (layout as fqb200_desc: outer x groups x inner, NCHW order; or channels_last != 0: [outer][inner][groups] memory,
  * groups % 4 == 0, 4 <= groups <= 2048) and the three candidate quantizers of get_alpha(clip_type='mix')
