@@ -161,6 +161,18 @@ def test_profile_mode():
     assert prof["modes"]["N"]["launches"] == 2
 
 
+def test_sum_of_squares_is_the_activation_norm():
+    """The activation norm kernels (`-ms`, ops.sample_sumsq, fq_measure.cuh) and column 1 of these sums without q add the
+    same float64 squares in the same order: bit for bit equal on the vector and the scalar path (DESIGN.md §4.6)."""
+    from cnn_quantization_b200 import ops
+    torch.manual_seed(4)
+    x = torch.randn(8, 64, 56, 56, device="cuda") * 3 + 0.5   # 13 chunks per row
+    misaligned = torch.randn(9 * 40000 + 1, device="cuda")[1:].view(9, 40000)
+    assert misaligned.data_ptr() % 16 != 0
+    for t in (x, x.contiguous(memory_format=torch.channels_last), misaligned):
+        assert torch.equal(ops.sample_sumsq(t), ops.sample_noise(t)[:, 1])
+
+
 # ---- the manager end to end -------------------------------------------------------------------------------------------------
 def batches():
     rs = np.random.RandomState(2026)   # make_noise_golden.py's batches
