@@ -1101,11 +1101,10 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 }  // namespace fqb
 #include "fq_cl.cuh"
 #include "fq_kld.cuh"
-#include "fq_measure.cuh"
 #include "fq_cliperr.cuh"
 #include "fq_kmeans.cuh"
 #include "fq_angle.cuh"
-#include "fq_noise.cuh"
+#include "fq_sample_sums.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -1683,41 +1682,60 @@ size_t kld_workspace(int64_t rows, int num_bins) {
   return align_up(static_cast<size_t>(rows) * 4, 256) + static_cast<size_t>(rows) * static_cast<size_t>(num_bins) * 4;
 }
 
-// sum-of-squares workspace: one float64 partial per (row, chunk) unit when a row spans several chunks (fq_measure.cuh)
-size_t sumsq_workspace(int64_t rows, int64_t row_len) {
-  const unsigned long long chunk = fqb::sumsq_chunk(static_cast<unsigned long long>(row_len));
+// per-sample sums workspace: `sums` float64 partials per (row, chunk) unit when a row spans several chunks
+// (fq_sample_sums.cuh)
+size_t sums_workspace(int64_t rows, int64_t row_len, int sums) {
+  const unsigned long long chunk = fqb::sums_chunk(static_cast<unsigned long long>(row_len));
   const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
-  return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * 8 : 0;
+  return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * static_cast<size_t>(sums) * 8 : 0;
+}
+
+// fq_sums_partial_kernel<VEC, S, BIAS>, then, when a row spans several chunks, fq_sums_finish_kernel<S>: the per-sample
+// sums of sum set S (1, 2 or 7) over rows x row_len; `what` names the launch in an error message
+template <int S>
+int launch_sums(const float* y, const float* q, const float* bias, int64_t bias_period, int64_t rows, int64_t row_len,
+                double* out, void* workspace, int32_t max_ctas, void* stream, const char* what) {
+  using namespace fqb;
+  DeviceInfo* di = nullptr;
+  const int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SumsArgs A;
+  memset(&A, 0, sizeof(A));
+  A.y = y;
+  A.q = q;
+  A.bias = bias;
+  A.period = static_cast<unsigned>(bias_period < 0 ? 0ull - static_cast<unsigned long long>(bias_period)
+                                                   : static_cast<unsigned long long>(bias_period));
+  A.rows = static_cast<unsigned long long>(rows);
+  A.row_len = static_cast<unsigned long long>(row_len);
+  A.chunk = sums_chunk(A.row_len);
+  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  const int grid = grid_for(A.rows * A.chunks, di->sms * (2048ull / kSumsThreads), max_ctas);
+  const bool vec = row_len % 4 == 0 && aligned16(y) && (!q || aligned16(q));
+#define FQB_LAUNCH_SUMS(B)                                                          \
+  do {                                                                              \
+    if (vec) fq_sums_partial_kernel<4, S, B><<<grid, kSumsThreads, 0, st>>>(A);     \
+    else     fq_sums_partial_kernel<1, S, B><<<grid, kSumsThreads, 0, st>>>(A);     \
+  } while (0)
+  if constexpr (S == 1) FQB_LAUNCH_SUMS(kSumsBiasNone);   // the activation norm takes no bias
+  else if (!bias) FQB_LAUNCH_SUMS(kSumsBiasNone);
+  else if (bias_period > 0) FQB_LAUNCH_SUMS(kSumsBiasNchw);
+  else FQB_LAUNCH_SUMS(kSumsBiasCl);
+#undef FQB_LAUNCH_SUMS
+  if (A.chunks > 1) {
+    const unsigned long long blocks = (A.rows * S + kSumsThreads - 1) / kSumsThreads;
+    fq_sums_finish_kernel<S><<<static_cast<unsigned>(blocks), kSumsThreads, 0, st>>>(A);
+  }
+  return launched(what);
 }
 
 // sample-angle workspace: one 64 x 64 float64 block per (tile pair, slice) unit (fq_angle.cuh)
 size_t angle_workspace(int64_t rows, int64_t row_len) {
   const fqb::AngleSplit s = fqb::angle_split(static_cast<unsigned long long>(rows), static_cast<unsigned long long>(row_len));
   return static_cast<size_t>(s.pairs * s.slices) * fqb::kAngTile * fqb::kAngTile * 8;
-}
-
-// quantization-noise workspace: kNoiseSums float64 partials per (row, chunk) unit when a row spans several chunks
-// (fq_noise.cuh; enough for the two sums of a call without q too)
-size_t noise_workspace(int64_t rows, int64_t row_len) {
-  const unsigned long long chunk = fqb::noise_chunk(static_cast<unsigned long long>(row_len));
-  const unsigned long long chunks = (static_cast<unsigned long long>(row_len) + chunk - 1) / chunk;
-  return chunks > 1 ? static_cast<size_t>(rows) * static_cast<size_t>(chunks) * fqb::kNoiseSums * 8 : 0;
-}
-
-// fq_noise_partial_kernel for a bias mode and with or without q
-template <int VEC>
-void launch_noise(int mode, bool q, int grid, cudaStream_t st, const fqb::NoiseArgs& A) {
-  using namespace fqb;
-  if (mode == kNoiseBiasNchw) {
-    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasNchw><<<grid, kNoiseThreads, 0, st>>>(A);
-    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasNchw><<<grid, kNoiseThreads, 0, st>>>(A);
-  } else if (mode == kNoiseBiasCl) {
-    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasCl><<<grid, kNoiseThreads, 0, st>>>(A);
-    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasCl><<<grid, kNoiseThreads, 0, st>>>(A);
-  } else {
-    if (q) fq_noise_partial_kernel<VEC, true, kNoiseBiasNone><<<grid, kNoiseThreads, 0, st>>>(A);
-    else   fq_noise_partial_kernel<VEC, false, kNoiseBiasNone><<<grid, kNoiseThreads, 0, st>>>(A);
-  }
 }
 
 // clipping-error workspace: kCeSums float64 partials per (group, unit) (fq_cliperr.cuh)
@@ -2446,7 +2464,7 @@ int fqb200_kld_threshold(const float* in, int64_t rows, int64_t row_len, int num
 size_t fqb200_sample_sumsq_workspace_bytes(int64_t rows, int64_t row_len) {
   g_err[0] = 0;
   if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s"), 0;
-  return sumsq_workspace(rows, row_len);
+  return sums_workspace(rows, row_len, 1);
 }
 
 int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* out, void* workspace, size_t workspace_bytes,
@@ -2454,30 +2472,11 @@ int fqb200_sample_sumsq(const float* in, int64_t rows, int64_t row_len, double* 
   g_err[0] = 0;
   if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s");
   if (!in || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
-  int rc = check_workspace(workspace, workspace_bytes, sumsq_workspace(rows, row_len), "fqb200_sample_sumsq_workspace_bytes");
+  const int rc = check_workspace(workspace, workspace_bytes, sums_workspace(rows, row_len, 1),
+                                 "fqb200_sample_sumsq_workspace_bytes");
   if (rc != FQB200_OK) return rc;
   if (rows == 0) return FQB200_OK;
-  DeviceInfo* di = nullptr;
-  rc = get_device(&di);
-  if (rc != FQB200_OK) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  fqb::SumsqArgs A;
-  memset(&A, 0, sizeof(A));
-  A.in = in;
-  A.rows = static_cast<unsigned long long>(rows);
-  A.row_len = static_cast<unsigned long long>(row_len);
-  A.chunk = fqb::sumsq_chunk(A.row_len);
-  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
-  A.partial = static_cast<double*>(workspace);
-  A.out = out;
-  const int grid = grid_for(A.rows * A.chunks, di->sms * (2048ull / fqb::kSumsqThreads));
-  if (row_len % 4 == 0 && aligned16(in)) fqb::fq_sumsq_partial_kernel<4><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
-  else                                   fqb::fq_sumsq_partial_kernel<1><<<grid, fqb::kSumsqThreads, 0, st>>>(A);
-  if (A.chunks > 1) {
-    const unsigned long long blocks = (A.rows + fqb::kSumsqThreads - 1) / fqb::kSumsqThreads;
-    fqb::fq_sumsq_finish_kernel<<<static_cast<unsigned>(blocks), fqb::kSumsqThreads, 0, st>>>(A);
-  }
-  return launched("sum-of-squares kernels");
+  return launch_sums<1>(in, nullptr, nullptr, 0, rows, row_len, out, workspace, 0, stream, "sum-of-squares kernels");
 }
 
 // the requests fqb200_sample_angles takes (FQB200_OK, or the code with the message in fqb200_last_error())
@@ -2533,7 +2532,7 @@ int fqb200_sample_angles(const float* in, int64_t rows, int64_t row_len, float* 
 size_t fqb200_sample_noise_workspace_bytes(int64_t rows, int64_t row_len) {
   g_err[0] = 0;
   if (rows < 0 || row_len <= 0) return fail(FQB200_ERR_INVALID, "rows must be >= 0 and row_len > 0%s"), 0;
-  return noise_workspace(rows, row_len);
+  return sums_workspace(rows, row_len, fqb::kSumsMax);   // enough for the two sums of a call without q too
 }
 
 int fqb200_sample_noise(const float* y, const float* q, const float* bias, int64_t bias_period, int64_t rows, int64_t row_len,
@@ -2550,36 +2549,13 @@ int fqb200_sample_noise(const float* y, const float* q, const float* bias, int64
     if (static_cast<unsigned long long>(row_len) > 0xffffffffull)
       return fail(FQB200_ERR_UNSUPPORTED, "rows of 2^32 elements and more take no bias%s");
   }
-  int rc = check_workspace(workspace, workspace_bytes, noise_workspace(rows, row_len), "fqb200_sample_noise_workspace_bytes");
+  const int rc = check_workspace(workspace, workspace_bytes, sums_workspace(rows, row_len, fqb::kSumsMax),
+                                 "fqb200_sample_noise_workspace_bytes");
   if (rc != FQB200_OK) return rc;
   if (rows == 0) return FQB200_OK;
-  DeviceInfo* di = nullptr;
-  rc = get_device(&di);
-  if (rc != FQB200_OK) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  fqb::NoiseArgs A;
-  memset(&A, 0, sizeof(A));
-  A.y = y;
-  A.q = q;
-  A.bias = bias;
-  A.period = static_cast<unsigned>(period);
-  A.rows = static_cast<unsigned long long>(rows);
-  A.row_len = static_cast<unsigned long long>(row_len);
-  A.chunk = fqb::noise_chunk(A.row_len);
-  A.chunks = (A.row_len + A.chunk - 1) / A.chunk;
-  A.sums = q ? fqb::kNoiseSums : 2;
-  A.partial = static_cast<double*>(workspace);
-  A.out = out;
-  const int grid = grid_for(A.rows * A.chunks, di->sms * (2048ull / fqb::kNoiseThreads), max_ctas);
-  const bool vec = row_len % 4 == 0 && aligned16(y) && (!q || aligned16(q));
-  const int mode = !bias ? fqb::kNoiseBiasNone : bias_period > 0 ? fqb::kNoiseBiasNchw : fqb::kNoiseBiasCl;
-  if (vec) launch_noise<4>(mode, q != nullptr, grid, st, A);
-  else     launch_noise<1>(mode, q != nullptr, grid, st, A);
-  if (A.chunks > 1) {
-    const unsigned long long blocks = (A.rows * A.sums + fqb::kNoiseThreads - 1) / fqb::kNoiseThreads;
-    fqb::fq_noise_finish_kernel<<<static_cast<unsigned>(blocks), fqb::kNoiseThreads, 0, st>>>(A);
-  }
-  return launched("quantization-noise kernels");
+  const char* what = "quantization-noise kernels";
+  if (q) return launch_sums<fqb::kSumsMax>(y, q, bias, bias_period, rows, row_len, out, workspace, max_ctas, stream, what);
+  return launch_sums<2>(y, nullptr, bias, bias_period, rows, row_len, out, workspace, max_ctas, stream, what);
 }
 
 // the layouts fqb200_clip_error takes (argument errors as a message, nullptr when they are fine)

@@ -500,22 +500,29 @@ def kld_threshold(x, num_bins=2001, num_quantized_bins=15, return_hist=False):
     return th, div, idx, ws[head:head + rows * num_bins * 4].view(torch.int32).view(rows, num_bins)
 
 
+def _sample_sums(entry, x, rows, row_len, shape, mode, bytes_per_elem, head, tail=()):
+    """The float64 ``shape`` device tensor the per-sample sums entry point ``entry`` writes for ``x`` (rows x row_len, from
+    ``_samples``), called as entry(*head, rows, row_len, out, workspace, workspace_bytes, *tail, stream) and recorded in
+    the launch profile under ``mode``."""
+    dev = x.device
+    if rows == 0 or x.numel() == 0:
+        return torch.zeros(shape, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
+    lib = L.load()
+    out = torch.empty(shape, dtype=torch.float64, device=dev)
+    need = getattr(lib, entry + "_workspace_bytes")(rows, row_len)
+    ws = _own_workspace(dev, need, required=False)
+    _launch(dev, _Timed(mode, x.numel(), bytes_per_elem, "%dx%d" % (rows, row_len)), getattr(lib, entry), *head, rows,
+            row_len, out.data_ptr(), _ptr(ws), need, *tail)
+    return out
+
+
 def sample_sumsq(x):
     """C ABI fqb200_sample_sumsq: ``x.double().pow(2).sum()`` of every sample (dim 0) of ``x`` as a float64 [N] device
     tensor - the activation norm `-ms` records (distance_stats.py:27-28).  Deterministic (fixed chunks, fixed summation
     order), no host synchronisation.  Recorded in the launch profile under mode 'M' (one read of the tensor), apart from
     the quantization launches."""
     x, rows, row_len = _samples(x, "sample_sumsq")
-    dev = x.device
-    if rows == 0 or x.numel() == 0:
-        return torch.zeros(rows, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
-    lib = L.load()
-    out = torch.empty(rows, dtype=torch.float64, device=dev)
-    need = lib.fqb200_sample_sumsq_workspace_bytes(rows, row_len)
-    ws = _own_workspace(dev, need, required=False)
-    _launch(dev, _Timed("M", x.numel(), 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_sumsq, x.data_ptr(), rows, row_len,
-            out.data_ptr(), _ptr(ws), need)
-    return out
+    return _sample_sums("fqb200_sample_sumsq", x, rows, row_len, (rows,), "M", 4, (x.data_ptr(),))
 
 
 def sample_angles(x, return_gram=False, max_ctas=0):
@@ -553,7 +560,6 @@ def sample_noise(y, q=None, bias=None, bias_period=0, max_ctas=0):
     channels-last one.  Deterministic (the bits depend neither on the run nor on ``max_ctas``), no host synchronisation.
     Recorded in the launch profile under mode 'N' (one read of y and q: 8 B/element, 4 without q)."""
     y, rows, row_len = _samples(y, "sample_noise")
-    dev = y.device
     if q is not None:
         _require_cuda_f32(q, "q")
         if q.shape != y.shape:
@@ -568,16 +574,8 @@ def sample_noise(y, q=None, bias=None, bias_period=0, max_ctas=0):
             raise ValueError("sample_noise: a bias of %d values on rows of %d elements needs bias_period %d (NCHW) or "
                              "%d (channels-last), got %d" % (c, row_len, row_len // max(c, 1), -c, period))
     shape = (rows, len(NOISE_SUMS) if q is not None else 2)
-    if rows == 0 or y.numel() == 0:
-        return torch.zeros(shape, dtype=torch.float64, device=dev)   # empty samples sum to 0, as in torch
-    out = torch.empty(shape, dtype=torch.float64, device=dev)
-    lib = L.load()
-    need = lib.fqb200_sample_noise_workspace_bytes(rows, row_len)
-    ws = _own_workspace(dev, need, required=False)
-    _launch(dev, _Timed("N", y.numel(), 8 if q is not None else 4, "%dx%d" % (rows, row_len)), lib.fqb200_sample_noise,
-            y.data_ptr(), _ptr(q), _ptr(bias), int(bias_period), rows, row_len, out.data_ptr(), _ptr(ws), need,
-            int(max_ctas))
-    return out
+    return _sample_sums("fqb200_sample_noise", y, rows, row_len, shape, "N", 8 if q is not None else 4,
+                        (y.data_ptr(), _ptr(q), _ptr(bias), int(bias_period)), (int(max_ctas),))
 
 
 CLIP_ERROR_CANDIDATES = ("lowp", "gaus", "laplace")

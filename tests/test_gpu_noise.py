@@ -162,8 +162,9 @@ def test_profile_mode():
 
 
 def test_sum_of_squares_is_the_activation_norm():
-    """The activation norm kernels (`-ms`, ops.sample_sumsq, fq_measure.cuh) and column 1 of these sums without q add the
-    same float64 squares in the same order: bit for bit equal on the vector and the scalar path (DESIGN.md §4.6)."""
+    """The activation norm (`-ms`, ops.sample_sumsq: the one-sum instance of fq_sample_sums.cuh) and column 1 of these sums
+    without q add the same float64 squares in the same order: bit for bit equal on the vector and the scalar path
+    (DESIGN.md §4.6)."""
     from cnn_quantization_b200 import ops
     torch.manual_seed(4)
     x = torch.randn(8, 64, 56, 56, device="cuda") * 3 + 0.5   # 13 chunks per row
