@@ -71,6 +71,9 @@ PROTOTYPES = {
     "fqb200_sample_sumsq_workspace_bytes": (_sz, [_i64, _i64]),
     "fqb200_clip_error": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _sz, _i32, _vp]),
     "fqb200_clip_error_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32]),
+    "fqb200_clip_mse": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _sz,
+                               _i32, _vp]),
+    "fqb200_clip_mse_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
     "fqb200_kmeans1d": (_i32, [_vp, _i64, _i32, _i64, _vp, _i32, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
                                _i32, _vp]),
     "fqb200_kmeans1d_workspace_bytes": (_sz, [_i64, _i32]),

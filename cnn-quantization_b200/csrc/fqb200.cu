@@ -1102,6 +1102,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_cl.cuh"
 #include "fq_kld.cuh"
 #include "fq_cliperr.cuh"
+#include "fq_clipmse.cuh"
 #include "fq_kmeans.cuh"
 #include "fq_angle.cuh"
 #include "fq_sample_sums.cuh"
@@ -1482,6 +1483,10 @@ void init_device(int dev) {
     return bad("KLD kernel setup", e);
   e = setup(fqb::fq_kmeans_kernel, fqb::kThreads, kmeans_smem(fqb::kKmMaxK));
   if (e != cudaSuccess) return bad("k-means kernel setup", e);
+  if ((e = setup(fqb::fq_clipmse_partial_kernel<0>, fqb::kCmThreads, fqb::cm_smem_bytes(fqb::kCmMaxK, 1))) != cudaSuccess ||
+      (e = setup(fqb::fq_clipmse_partial_kernel<1>, fqb::kCmThreads, fqb::cm_smem_bytes(fqb::kCmMaxK, 1))) != cudaSuccess ||
+      (e = setup(fqb::fq_clipmse_partial_kernel<2>, fqb::kCmThreads, fqb::cm_smem_bytes(fqb::kCmMaxK, fqb::kCmSlab))) != cudaSuccess)
+    return bad("clipping-MSE kernel setup", e);
   // mid-tread table (int_quantizer.py:41-51): omega grid = 5 decades x 20 steps, leading 0
   double om[fqb::kTable], al[fqb::kTable];
   om[0] = 0.0;
@@ -1746,6 +1751,17 @@ unsigned long long cliperr_units_per_group(int64_t outer, int64_t inner, int cha
 }
 size_t cliperr_workspace(int64_t outer, int64_t groups, int64_t inner, int channels_last) {
   return static_cast<size_t>(groups) * static_cast<size_t>(cliperr_units_per_group(outer, inner, channels_last)) * fqb::kCeSums * 8;
+}
+
+// clipping-MSE workspace: K + 1 float64 partials per (group, unit) (fq_clipmse.cuh)
+unsigned long long clipmse_units_per_group(int64_t outer, int64_t inner, int channels_last) {
+  const unsigned long long n = static_cast<unsigned long long>(outer) * static_cast<unsigned long long>(inner);
+  const unsigned long long per = channels_last ? fqb::kCmClRows : fqb::kCmChunk;
+  return (n + per - 1) / per;
+}
+size_t clipmse_workspace(int64_t outer, int64_t groups, int64_t inner, int channels_last, int k) {
+  return static_cast<size_t>(groups) * static_cast<size_t>(clipmse_units_per_group(outer, inner, channels_last)) *
+         static_cast<size_t>(k + 1) * 8;
 }
 
 // k-means workspace (fq_kmeans.cuh): barrier words, control block, per-block / per-superblock column sums, Lloyd unit
@@ -2613,6 +2629,74 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
   else                                                   fqb::fq_cliperr_partial_kernel<1><<<grid, fqb::kCeThreads, 0, st>>>(A);
   fqb::fq_cliperr_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCeThreads, 0, st>>>(A);
   return launched("clipping-error kernels");
+}
+
+// the layouts and candidate counts fqb200_clip_mse takes (argument errors as a message, nullptr when they are fine)
+static const char* clipmse_bad_args(int64_t outer, int64_t groups, int64_t inner, int channels_last, int32_t k) {
+  const char* bad = cliperr_bad_args(outer, groups, inner, channels_last);
+  if (bad) return bad;
+  if (k < 1 || k > fqb::kCmMaxK) return "num_multipliers must be in 1..256%s";
+  return nullptr;
+}
+
+size_t fqb200_clip_mse_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                                       int32_t num_multipliers) {
+  g_err[0] = 0;
+  const char* bad = clipmse_bad_args(outer, groups, inner, channels_last, num_multipliers);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  return clipmse_workspace(outer, groups, inner, channels_last, num_multipliers);
+}
+
+int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last, const float* stats,
+                    int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, int32_t prior,
+                    const float* multipliers, int32_t num_multipliers, double* out, float* out_params, void* workspace,
+                    size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  const char* bad = clipmse_bad_args(outer, groups, inner, channels_last, num_multipliers);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!in || !stats || !multipliers || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
+  if (bit_alloc && num_bits > 4) return fail(FQB200_ERR_INVALID, "bit_alloc applies to num_bits <= 4 only%s");
+  if (prior != 0 && prior != 1) return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b) or 1 (Gauss std)%s");
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  int rc = check_workspace(workspace, workspace_bytes, clipmse_workspace(outer, groups, inner, channels_last, num_multipliers),
+                           "fqb200_clip_mse_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  DeviceInfo* di = nullptr;
+  rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::ClipMseArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.stats = stats;
+  A.mult = multipliers;
+  A.outer = static_cast<unsigned long long>(outer);
+  A.groups = static_cast<unsigned long long>(groups);
+  A.inner = static_cast<unsigned long long>(inner);
+  A.channels_last = channels_last ? 1 : 0;
+  A.num_bits = num_bits;
+  A.positive = positive ? 1 : 0;
+  A.bit_alloc = bit_alloc ? 1 : 0;
+  A.solve_f64 = solve_f64 ? 1 : 0;
+  A.prior = prior;
+  A.K = num_multipliers;
+  A.Kpad = (num_multipliers + fqb::kCmTile - 1) / fqb::kCmTile * fqb::kCmTile;
+  A.units_per_group = clipmse_units_per_group(outer, inner, channels_last);
+  A.units = A.units_per_group * (channels_last ? (A.groups + fqb::kCmSlab - 1) / fqb::kCmSlab : A.groups);
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  A.params = out_params;
+  const int grid = grid_for(A.units, di->sms * 2ull, max_ctas);
+  if (channels_last) {
+    fqb::fq_clipmse_partial_kernel<2><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, fqb::kCmSlab), st>>>(A);
+  } else if (inner % 4 == 0 && aligned16(in)) {
+    fqb::fq_clipmse_partial_kernel<1><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
+  } else {
+    fqb::fq_clipmse_partial_kernel<0><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
+  }
+  fqb::fq_clipmse_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCmThreads, 0, st>>>(A);
+  return launched("clipping-MSE kernels");
 }
 
 // the requests fqb200_kmeans1d takes (argument errors as a message, nullptr when they are fine)

@@ -94,6 +94,8 @@ class IntQuantizer(object):
         # singleton CLASS here, inference_quantization_manager.py:413,450,464,471; any object with
         # get_tensor_stat(id, stat, kind) works)
         self.sm = None
+        # `-c mse`: the statistics.ClipMseStatistics that reads the collected clipping-MSE curves (set by the manager)
+        self.mse_curves = None
         self._stat_cache = {}  # offline-statistics parameters are constants of a layer: solved once, kept on the device
         self.force_positive = False
         self.half_range = False
@@ -399,6 +401,8 @@ class IntQuantizer(object):
             per_channel = pc_shape and np.size(mn) > 1 and np.size(mx) > 1
             if clip_type == "mix":
                 alpha, bits = self._mix_alpha_from_stats(stat_id, per_channel, dev)
+            elif clip_type == "mse":
+                alpha, bits = self._mse_alpha_from_stats(stat_id, per_channel, dev)
             else:
                 alpha, bits = self._alpha_from_stats(stat_id, clip_type, per_channel, dev)
             if per_channel:
@@ -464,6 +468,28 @@ class IntQuantizer(object):
         if bits is None and self.bit_alloc_act and per_channel and self.num_bits <= 4:
             bits = self._stat_bits(stat_id, dev, self.bit_alloc_target_act)
         return alpha, bits
+
+    def _mse_alpha_from_stats(self, stat_id, per_channel, dev):
+        """`-c mse`: per group, alpha = m* times the summary b (or std, for curves collected with mse_prior="gaus"), m* the
+        multiplier at the minimum of the group's collected clipping-MSE curve (ties: the smaller multiplier) - in fp32 per
+        channel, in float64 per tensor, like the Laplace alpha.  Bits as in `-c laplace`."""
+        if self.mse_curves is None:
+            raise KeyError("-c mse needs the clipping-MSE curve of layer %r: collect it with collect_mse=True" % (stat_id,))
+        m, prior = self.mse_curves.best(stat_id)
+        scale = self._stat(stat_id, "b" if prior == "laplace" else "std", "mean")
+        bits = None
+        if per_channel:
+            scale = np.asarray(scale, dtype=np.float32).reshape(-1)
+            if m.size not in (1, scale.size):
+                raise ValueError("-c mse: the curve of %r has %d groups, the statistics %d channels" % (stat_id, m.size, scale.size))
+            alpha = scale * m
+            if self.bit_alloc_act and self.num_bits <= 4:
+                bits = self._stat_bits(stat_id, dev, self.bit_alloc_target_act)
+            return alpha, bits
+        if m.size != 1:
+            raise ValueError("-c mse: the curve of %r is per channel (%d groups) but the layer is quantized per tensor"
+                             % (stat_id, m.size))
+        return float(scale) * float(m[0]), bits
 
     # ------------------------------------------------------------------------------------------
     # dispatch targets
@@ -843,12 +869,18 @@ class IntQuantizer(object):
         return p * stats(tensor, ["std"])["std"]
 
     def get_alpha(self, tensor, tag="", stat_id=None, clip_type="laplace", per_channel=False):
-        """int_quantizer.py:302-325.  ``mix`` needs collected statistics (``stat_id`` and ``sm``), as in the reference."""
+        """int_quantizer.py:302-325.  ``mix`` needs collected statistics (``stat_id`` and ``sm``), as in the reference;
+        so does ``mse``, this package's extension."""
         if clip_type == "mix":
             if stat_id is None or self.sm is None:
                 raise NotImplementedError("clipping 'mix' chooses by collected errors: it needs stat_id and a statistics "
                                           "manager (-sm use with statistics collected with collect_err=True)")
             return self._mix_alpha_from_stats(stat_id, per_channel, tensor.device)[0]
+        if clip_type == "mse":
+            if stat_id is None or self.sm is None:
+                raise NotImplementedError("clipping 'mse' clips at the minimum of collected curves: it needs stat_id and a "
+                                          "statistics manager (-sm use with curves collected with collect_mse=True)")
+            return self._mse_alpha_from_stats(stat_id, per_channel, tensor.device)[0]
         if clip_type == "laplace":
             return self.get_alpha_laplace(tensor, stat_id, per_channel=per_channel)
         if clip_type == "gaus":

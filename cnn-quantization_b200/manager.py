@@ -32,7 +32,10 @@ FUSED_RELU_ARCHS = ("alexnet", "vgg16", "vgg16_bn", "inception_v3")
 def make_args(**over):
     """An ``args`` namespace with the reference CLI's defaults (inference/inference_sim.py:52-112) for the fields the
     manager and the quantizers read.  Extensions without a reference flag: ``stats_base_dir``, ``collect_err`` (fill the
-    mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument) and
+    mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument), ``collect_mse`` (also
+    write the clipping-MSE curve of every call site's quantizer in `-sm collect`, over ``mse_multipliers`` - default
+    statistics.MSE_MULTIPLIERS, 0.5 .. 16 in steps of 0.125 - times the Laplace b or, with ``mse_prior="gaus"``, the std;
+    `-c mse` in use mode clips at the minimum of those curves) and
     ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms; "angle", the
     pairwise sample angles of its angle_stats module, which the reference selects by editing an import; or "noise", the
     per-sample quantization error statistics of its measure_statistics module, which the reference cannot run)."""
@@ -42,7 +45,7 @@ def make_args(**over):
              bit_alloc_rmode="round", bit_alloc_prior="gaus", bit_alloc_target_act=None, bit_alloc_target_weight=None,
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
              mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
-             collect_err=False, measure_stats_kind="distance")
+             collect_err=False, measure_stats_kind="distance", collect_mse=False, mse_multipliers=None, mse_prior="laplace")
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -404,6 +407,12 @@ class QuantizationManagerInference(object):
         if self.collect_err and (self.stats_mode != "collect" or args.qtype is None):
             raise ValueError("collect_err fills error columns of -sm collect for the bit widths of -qtype: it needs "
                              "stats_mode='collect' and a qtype (got stats_mode=%r, qtype=%r)" % (self.stats_mode, args.qtype))
+        # `collect_mse`: the collect hooks also measure each tensor's clipping-MSE curve with the same quantizer settings
+        self.collect_mse = bool(getattr(args, "collect_mse", False))
+        if self.collect_mse and (self.stats_mode != "collect" or args.qtype is None):
+            raise ValueError("collect_mse measures the clipping-MSE curves of -sm collect for the bit widths of -qtype: it "
+                             "needs stats_mode='collect' and a qtype (got stats_mode=%r, qtype=%r)" % (self.stats_mode, args.qtype))
+        self.clip_mse = None
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None
         self._sm_tensor = self._sm_channel = None
@@ -421,10 +430,17 @@ class QuantizationManagerInference(object):
                 else:
                     self.stats_manager = StatisticManager(sf, load_stats=False, kld_threshold=args.kld_threshold,
                                                           batch_avg=args.stats_batch_avg, base_dir=base)
+                if self.collect_mse:
+                    from .statistics import ClipMseStatistics
+                    self.clip_mse = ClipMseStatistics(sf, getattr(args, "mse_multipliers", None),
+                                                      getattr(args, "mse_prior", "laplace"), base_dir=base)
             else:
                 if args.per_channel_quant_act:
                     self._sm_channel = StatisticManagerPerChannel(sf, load_stats=True, base_dir=base)
                 self._sm_tensor = StatisticManager(sf, load_stats=True, base_dir=base)
+                if args.clipping == "mse":   # read on first use: a missing file raises KeyError naming collect_mse there
+                    from .statistics import ClipMseStatistics
+                    self.clip_mse = ClipMseStatistics(sf, base_dir=base, load=True)
         self.fused_relu = args.arch is not None and (args.arch in FUSED_RELU_ARCHS or "squeezenet" in args.arch)
         self.ignore_ids = []
         self.quantizers = {}
@@ -448,6 +464,7 @@ class QuantizationManagerInference(object):
                     if isinstance(q, DummyQuantizer):
                         continue
                     q.sm = per_channel if tag in ("activation", "weight", "weight_classifier", "") else per_tensor
+                    q.mse_curves = self.clip_mse
             if self.inplace_activations:
                 for tag, q in list(self.quantizers.items()) + [("", self.quantizer_default)]:
                     if tag.startswith("activation") or tag in ("", "ignored"):
@@ -543,6 +560,8 @@ class QuantizationManagerInference(object):
         self.detach()
         if self.stats_manager is not None:
             self.stats_manager.__exit__()  # collect mode: write the CSV / pickle files
+        if self.clip_mse is not None:
+            self.clip_mse.__exit__()       # collect_mse: clip_mse.pkl and curve.csv
         if self.measure_stats is not None:
             self.measure_stats.__exit__()  # -ms: write distance.csv (angle.pkl, noise/<id>.csv with the other kinds)
 
@@ -676,20 +695,24 @@ class QuantizationManagerInference(object):
 
         return measured
 
-    def _clip_err(self, out, tag, stat_id, half_range):
+    def _clip_err(self, out, tag, stat_id, half_range, name):
         """``save_tensor_stats`` kwargs of a collect call site: with collect_err, the settings of the quantizer
         quantize_instant picks for the same call in `-sm use` (``tag``, the 8-bit ``ignored`` list, ``half_range``) on
-        this tensor ``out``: per channel when it would quantize it per channel, with bit allocation only then."""
-        if not self.collect_err:
+        this tensor ``out``: per channel when it would quantize it per channel, with bit allocation only then.  With
+        collect_mse, the call site's clipping-MSE curve is measured here, with the same settings (``name``: the
+        internal name save_tensor_stats records)."""
+        if not (self.collect_err or self.collect_mse):
             return {}
         from .statistics import ClipErrConfig
         q = self.get_quantizer("ignored" if stat_id in self.ignore_ids else tag)
         per_channel = bool(q.pcq_a and out.dim() == 4 and (out.shape[2] > 1 or out.shape[3] > 1) and out.shape[1] > 1)
-        return {"clip_err": ClipErrConfig(num_bits=min(q.num_bits, 8), positive=bool(q.force_positive or half_range),
-                                          per_channel=per_channel,
-                                          bit_alloc=bool(per_channel and q.bit_alloc_act and q.num_bits <= 4),
-                                          bit_alloc_prior=L.PRIOR_STD if q.bit_alloc_prior == "gaus" else L.PRIOR_B,
-                                          bit_alloc_round=bool(q.bit_alloc_round), bit_alloc_target=q.bit_alloc_target_act)}
+        cfg = ClipErrConfig(num_bits=min(q.num_bits, 8), positive=bool(q.force_positive or half_range),
+                            per_channel=per_channel, bit_alloc=bool(per_channel and q.bit_alloc_act and q.num_bits <= 4),
+                            bit_alloc_prior=L.PRIOR_STD if q.bit_alloc_prior == "gaus" else L.PRIOR_B,
+                            bit_alloc_round=bool(q.bit_alloc_round), bit_alloc_target=q.bit_alloc_target_act)
+        if self.collect_mse:
+            self.clip_mse.save_curve(out, name, stat_id, cfg)
+        return {"clip_err": cfg} if self.collect_err else {}
 
     def _stat_id(self, activation_id):
         return activation_id if self.stats_mode == "use" else None
@@ -702,8 +725,9 @@ class QuantizationManagerInference(object):
         tag = "activation_classifier" if out.shape[1] == 1000 else "activation"
         half_range = hasattr(m, "before_relu")
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, getattr(m, "internal_name", activation_id), activation_id,
-                                                 **self._clip_err(out, tag, activation_id, half_range))
+            name = getattr(m, "internal_name", activation_id)
+            self.stats_manager.save_tensor_stats(out, name, activation_id,
+                                                 **self._clip_err(out, tag, activation_id, half_range, name))
             return None
         extra = {} if bias is None else {"bias": bias}
         if self.stats_mode == "use" and self.bcorr_act:
@@ -755,7 +779,7 @@ class QuantizationManagerInference(object):
         half_range = hasattr(m, "before_relu") if not classifier else False
         if self.stats_mode == "collect":
             self.stats_manager.save_tensor_stats(out, tag, activation_id, force_global_min_max=("classifier" in tag),
-                                                 **self._clip_err(out, tag, activation_id, half_range))
+                                                 **self._clip_err(out, tag, activation_id, half_range, tag))
             return None
         return self.quantize_instant(out, activation_id, tag, stat_id=self._stat_id(activation_id), half_range=half_range,
                                      verbose=self.verbose)
@@ -766,7 +790,8 @@ class QuantizationManagerInference(object):
         out_id = "maxpool%d_out" % m._fq_id
         if self.stats_mode == "collect":
             self.stats_manager.save_tensor_stats(out, "activation_pooling", out_id,
-                                                 **self._clip_err(out, "activation_pooling", out_id, False))
+                                                 **self._clip_err(out, "activation_pooling", out_id, False,
+                                                                  "activation_pooling"))
             return None
         return self.quantize_instant(out, out_id, "activation_pooling", stat_id=self._stat_id(out_id), verbose=self.verbose)
 
@@ -776,7 +801,7 @@ class QuantizationManagerInference(object):
         out_id = "avgpool%d_out" % m._fq_id
         tag_act = "activation_classifier" if out.shape[1] == 1000 else "activation_pooling"
         if self.stats_mode == "collect":
-            self.stats_manager.save_tensor_stats(out, tag_act, out_id, **self._clip_err(out, "", out_id, False))
+            self.stats_manager.save_tensor_stats(out, tag_act, out_id, **self._clip_err(out, "", out_id, False, tag_act))
             return None
         # the reference passes the tag in the id slot here (:96,:99): the tensor goes through the DEFAULT quantizer
         return self.quantize_instant(out, tag_act, stat_id=self._stat_id(out_id), verbose=self.verbose)
@@ -789,7 +814,8 @@ class QuantizationManagerInference(object):
         activation_id = "bn%d_activation" % m._fq_id
         if self.stats_mode == "collect":
             self.stats_manager.save_tensor_stats(out, "activation", activation_id,
-                                                 **self._clip_err(out, "", activation_id, hasattr(m, "before_relu")))
+                                                 **self._clip_err(out, "", activation_id, hasattr(m, "before_relu"),
+                                                                  "activation"))
             return None
         # same argument-order slip as the reference (:275,:278): id="activation", tag="" -> default quantizer
         return self.quantize_instant(out, "activation", stat_id=self._stat_id(activation_id),

@@ -25,8 +25,8 @@ def profile_collect():
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
     (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'N' the quantization-noise measurement
-    (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error) and 'C' the k-means clustering of a weight
-    tensor (ops.kmeans1d), which quantize nothing."""
+    (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error), 'R' the clipping-MSE curves (ops.clip_mse)
+    and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -621,7 +621,56 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
     return (out, params) if want_params else out
 
 
-KMeans1d = collections.namedtuple("KMeans1d", "labels centres inertia n_iter init_ids out out_bcorr")
+CLIP_MSE_PRIORS = {"laplace": 0, "gaus": 1}
+
+
+def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, prior="laplace", bit_alloc=False,
+             solve_f64=None, want_params=False, max_ctas=0):
+    """C ABI fqb200_clip_mse: per group of ``layout`` = (outer, groups, inner), the clipping-MSE curve of the quantizer
+    ``clip_error`` describes, over K = len(``multipliers``) (1..256) clipping values alpha_k = multipliers[k] * b
+    (``prior`` "laplace") or * std ("gaus"), as a [groups, K + 1] float64 device tensor: column 0 sum x^2, column 1 + k
+    sum (x - q_k)^2.  ``table``, ``channels_last``, ``bit_alloc`` and ``solve_f64`` as in ``clip_error``; a multiplier equal
+    to the ACIQ Laplace factor of the width gives its Laplace candidate.  ``multipliers``: a sequence of floats or a
+    float32 tensor (rounded to float32).  Deterministic, no host synchronisation; with ``want_params`` also returns the
+    [groups, K, 6] candidate parameters (delta, offset, bits, scale, zero point, qmax).  Recorded in the launch profile
+    under mode 'R' (one read of the tensor)."""
+    _require_cuda_f32(x, "tensor")
+    outer, groups, inner = (int(v) for v in layout)
+    if outer * groups * inner != x.numel():
+        raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
+    if prior not in CLIP_MSE_PRIORS:
+        raise ValueError("prior must be one of %s, got %r" % (sorted(CLIP_MSE_PRIORS), prior))
+    if channels_last:
+        if not cl_eligible(x, layout):
+            raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
+    elif not (outer == 1 and groups == 1 and dense(x)):
+        x = x.contiguous()   # one group: any dense memory order; per channel: NCHW order
+    if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
+            or tuple(table.shape) != (groups, L.STATS_STRIDE)):
+        raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
+    table = table.contiguous()
+    mult = torch.as_tensor(multipliers, dtype=torch.float32).reshape(-1).to(x.device).contiguous()
+    k = mult.numel()
+    if not 1 <= k <= 256:
+        raise ValueError("clip_mse takes 1..256 multipliers, got %d" % k)
+    lib = L.load()
+    dev = x.device
+    if solve_f64 is None:
+        solve_f64 = groups == 1
+    out = torch.empty((groups, k + 1), dtype=torch.float64, device=dev)
+    params = torch.empty((groups, k, 6), dtype=torch.float32, device=dev) if want_params else None
+    if x.numel() == 0:
+        out.zero_()
+        return (out, params) if want_params else out
+    ws = _own_workspace(dev, lib.fqb200_clip_mse_workspace_bytes(outer, groups, inner, int(bool(channels_last)), k))
+    _launch(dev, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse, x.data_ptr(), outer,
+            groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), int(bool(bit_alloc)),
+            int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), k, out.data_ptr(), _ptr(params), ws.data_ptr(),
+            ws.numel(), int(max_ctas))
+    return (out, params) if want_params else out
+
+
+KMeans1d =collections.namedtuple("KMeans1d", "labels centres inertia n_iter init_ids out out_bcorr")
 KMEANS_TASKS = {None: 0, "quantize": 1, "clip": 2}
 
 

@@ -40,6 +40,17 @@ quantizer put into its output, with the moments of the layer's input, output and
 
 Each hooked tensor costs two ops.sample_noise launch pairs (output with its quantized form, input) and each weight one,
 once; the float64 sums stay on the device until ``__exit__`` (72 B per sample and call).
+
+``ClipMseStatistics`` is the clipping-MSE curve of every collect call site (`collect_mse`; the simulation of the
+reference's mse_analysis.py on real activations, with the quantizer the call site uses in `-sm use`), and what `-c mse`
+reads back in use mode:
+
+    <base>/clip_mse/<folder>/clip_mse.pkl   {"multipliers", "prior", id: DataFrame[count, b, std, bits, mse_<k>...], one
+                                            row per group (channel of a per-channel quantizer, else the whole tensor)}
+    <base>/clip_mse/<folder>/curve.csv      id, internal_name, multiplier, mse, mse_laplace_analytic, mse_gaus_analytic
+
+Each hooked tensor costs one statistics-only launch and one ops.clip_mse launch pair; the sums stay on the device until
+``__exit__``, which reads everything back in one copy.
 """
 import collections
 import os
@@ -53,7 +64,7 @@ import torch
 from . import ops
 
 __all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "AngleStatistics", "NoiseStatistics",
-           "ClipErrConfig", "default_base_dir"]
+           "ClipErrConfig", "ClipMseStatistics", "MSE_MULTIPLIERS", "default_base_dir"]
 
 
 def default_base_dir():
@@ -530,3 +541,149 @@ class NoiseStatistics(object):
         for id, table in tables.items():
             pd.DataFrame(columns=NOISE_COLUMNS, data=table).to_csv(os.path.join(self.folder, "%s.csv" % id), index=False)
         self.stats, self.weights = {}, {}
+
+
+MSE_MULTIPLIERS = tuple(0.5 + 0.125 * k for k in range(125))   # clipping values 0.5 .. 16 times b (or std)
+
+
+def _clip_table(t, cfg, channels_last):
+    """(layout, stats table) of the on-the-fly launch of the quantizer ``cfg`` describes on ``t``: per channel (with
+    the bit allocation's widths) or over the whole tensor."""
+    if not cfg.per_channel:
+        layout = (1, 1, t.numel())
+        return layout, ops.fused(t, layout, stats_only=True, any_dense_format=True)
+    n, c = t.shape[0], t.shape[1]
+    layout = (n, c, t.numel() // (n * c))
+    return layout, ops.fused(t, layout, num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
+                             bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
+                             bit_alloc_target=cfg.bit_alloc_target, stats_only=True, channels_last=channels_last)
+
+
+def best_multipliers(multipliers, mse):
+    """Per row of ``mse`` ([G, K], one column per multiplier) the multiplier of the smallest MSE; ties go to the smaller
+    multiplier and NaN never wins (a row of NaN gives the smallest multiplier)."""
+    m = np.asarray(multipliers, dtype=np.float32)
+    order = np.argsort(m, kind="stable")
+    e = np.asarray(mse, dtype=np.float64)[:, order]
+    e = np.where(np.isnan(e), np.inf, e)
+    return m[order][np.argmin(e, axis=1)]
+
+
+class ClipMseStatistics(object):
+    """Clipping-MSE curves (`collect_mse`): ``save_curve(t, tag, id, cfg)`` adds, per group of the quantizer ``cfg`` (a
+    ClipErrConfig, as collect_err passes) describes, the float64 sums of ops.clip_mse over ``multipliers`` (alpha = m * b
+    with prior "laplace", m * std with "gaus") and the group's b, std and width to device accumulators; ``__exit__``
+    writes clip_mse.pkl and curve.csv.  With ``load`` the instance reads clip_mse.pkl instead (on first use), for `-c mse`.
+
+    curve.csv holds layer totals per element: mse = sum_g sum (x - q)^2 / sum_g count, and the reference's analytic
+    curves (mse_analysis.py) per group at the same alpha, with that group's b or std and width (width + 1 for a positive
+    range, the relation the reference's *_positive ACIQ tables encode), weighted by the group's count."""
+
+    def __init__(self, folder, multipliers=None, prior="laplace", base_dir=None, load=False):
+        if prior not in ops.CLIP_MSE_PRIORS:
+            raise ValueError("mse_prior must be one of %s, got %r" % (sorted(ops.CLIP_MSE_PRIORS), prior))
+        self.folder = os.path.join(base_dir or default_base_dir(), "clip_mse", folder)
+        self.multipliers = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers, dtype=np.float32).reshape(-1)
+        if not 1 <= self.multipliers.size <= 256:
+            raise ValueError("mse_multipliers: 1..256 values, got %d" % self.multipliers.size)
+        self.prior = prior
+        self.load = load
+        self.curves = None
+        self.acc = {}    # id -> (sums [G, K + 1], b / std / bits sums [G, 3], float64 device tensors, batches)
+        self.meta = {}   # id -> (internal_name, positive, elements per group and batch)
+        self._mult_dev = {}
+
+    # -- collect ---------------------------------------------------------------------------------------------------
+    def save_curve(self, tensor, tag, id, cfg):
+        t = tensor.detach()
+        if cfg.per_channel:
+            n, c = t.shape[0], t.shape[1]
+            cl = ops.cl_eligible(t, (n, c, t.numel() // (n * c)))
+        else:
+            cl = False
+        if not (cl or (ops.dense(t) and not cfg.per_channel)):
+            t = t.contiguous()   # per channel: NCHW order; one group: any dense memory order
+        layout, table = _clip_table(t, cfg, cl)
+        mult = self._mult_dev.get(t.device)
+        if mult is None:
+            mult = self._mult_dev[t.device] = torch.from_numpy(self.multipliers).to(t.device)
+        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=self.prior,
+                            bit_alloc=cfg.bit_alloc, solve_f64=not cfg.per_channel)
+        bits = table[:, 7] if cfg.bit_alloc else torch.full_like(table[:, 7], float(cfg.num_bits))
+        scales = torch.stack([table[:, 3], table[:, 4], bits], 1).double()
+        prev = self.acc.get(id)
+        if prev is None:
+            self.acc[id] = (sums, scales, 1)
+            self.meta[id] = (tag, bool(cfg.positive), layout[0] * layout[2])
+        else:
+            if prev[0].shape != sums.shape:
+                raise ValueError("collect_mse of %r: %d groups in this call, %d before" % (id, sums.shape[0], prev[0].shape[0]))
+            self.acc[id] = (prev[0] + sums, prev[1] + scales, prev[2] + 1)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *args):
+        if self.load or not self.acc:
+            return
+        import pandas as pd
+        from . import mse_analysis
+        ids = list(self.acc)
+        flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
+        k = self.multipliers.size
+        mults = self.multipliers.astype(np.float64)
+        out = {"multipliers": mults, "prior": self.prior}
+        rows = []
+        pos = 0
+        for id in ids:
+            sums, scales, batches = self.acc[id]
+            g = sums.shape[0]
+            s = flat[pos:pos + g * (k + 1)].reshape(g, k + 1)
+            pos += g * (k + 1)
+            sc = flat[pos:pos + g * 3].reshape(g, 3) / batches
+            pos += g * 3
+            tag, positive, per_batch = self.meta[id]
+            count = np.full(g, float(per_batch * batches))
+            mse = s[:, 1:] / count[:, None]
+            df = pd.DataFrame({"count": count, "b": sc[:, 0], "std": sc[:, 1], "bits": sc[:, 2]})
+            df = pd.concat([df, pd.DataFrame(mse, columns=["mse_%d" % j for j in range(k)])], axis=1)
+            out[id] = df
+            width = sc[:, 2] + (1 if positive else 0)
+            scale = sc[:, 0] if self.prior == "laplace" else sc[:, 1]
+            lap = np.empty((g, k))
+            gau = np.empty((g, k))
+            for r in range(g):
+                alpha = mults * scale[r]
+                lap[r] = mse_analysis.LaplacianClippingAnalysis(alpha, float(sc[r, 0]), float(width[r])).numpy()
+                gau[r] = mse_analysis.GaussianClippingAnalysis(alpha, float(sc[r, 1]), float(width[r])).numpy()
+            total = count.sum()
+            layer = s[:, 1:].sum(0) / total
+            with np.errstate(invalid="ignore", divide="ignore"):
+                lap_t = (count[:, None] * lap).sum(0) / total
+                gau_t = (count[:, None] * gau).sum(0) / total
+            for j in range(k):
+                rows.append((id, tag, mults[j], layer[j], lap_t[j], gau_t[j]))
+        if os.path.exists(self.folder):
+            shutil.rmtree(self.folder)
+        os.makedirs(self.folder)
+        with open(os.path.join(self.folder, "clip_mse.pkl"), "wb") as f:
+            pickle.dump(out, f)
+        pd.DataFrame(rows, columns=["id", "internal_name", "multiplier", "mse", "mse_laplace_analytic",
+                                    "mse_gaus_analytic"]).to_csv(os.path.join(self.folder, "curve.csv"), index=False)
+        self.acc, self.meta = {}, {}
+
+    # -- use (`-c mse`) ----------------------------------------------------------------------------------------------
+    def best(self, id):
+        """(m* per group as float32 [G], prior) of the curve collected for ``id``; KeyError naming collect_mse when there
+        is none."""
+        if self.curves is None:
+            path = os.path.join(self.folder, "clip_mse.pkl")
+            if not os.path.exists(path):
+                raise KeyError("-c mse needs the clipping-MSE curves at %s: collect them with collect_mse=True" % path)
+            with open(path, "rb") as f:
+                self.curves = pickle.load(f)
+        df = self.curves.get(id)
+        if df is None:
+            raise KeyError("-c mse needs the clipping-MSE curve of layer %r: collect it with collect_mse=True" % (id,))
+        m = self.curves["multipliers"]
+        return best_multipliers(m, df[["mse_%d" % j for j in range(len(m))]].to_numpy()), self.curves["prior"]

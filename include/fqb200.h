@@ -368,6 +368,33 @@ int fqb200_clip_error(const float* in, int64_t outer, int64_t groups, int64_t in
 size_t fqb200_clip_error_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last);
 
 /*
+ * Clipping-MSE curves (the simulation of the reference's mse_analysis.py, eq. 6 of the paper, on real tensors): for every
+ * group g of x (layouts as fqb200_clip_error) and K = num_multipliers (1..256) candidate quantizers that differ only in
+ * their clipping value, out[g * (K + 1) + j] =
+ *   j = 0: sum x^2;  j = 1 + k: sum (x - q_k)^2     (float64, x - q_k formed in float64)
+ * where candidate k clips at alpha = multipliers[k] * b (prior 0, the Laplace scale, column 3 of `stats`) or
+ * multipliers[k] * std (prior 1, Gauss, column 4), one fp32 multiply, and q_k is the torch leaf with the parameters
+ * solve_range gives that alpha from `stats` (a stats_only fqb200_fused table on the same x), exactly as fqb200_clip_error
+ * solves its candidates: float64 alpha2DeltaOffset when solve_f64, else fp32; the positive range when `positive`; num_bits
+ * (1..8) or, with bit_alloc (num_bits <= 4), the table's allocated widths.  A multiplier equal to the ACIQ Laplace factor of
+ * the width gives fqb200_clip_error's Laplace candidate.  `multipliers` is a device array of K floats.  out_params
+ * (optional, [groups][K][6] floats): per candidate delta, offset, bits, scale, zero point, qmax.  One read of x
+ * (4 B/element) and a small second launch on `stream`; nothing else is written, no host synchronisation.  Work units and
+ * summation order are fixed (no atomics on values): the bits do not depend on the run or on max_ctas (0: the default
+ * grid, else at most that many CTAs).  NaN propagates.  The workspace (fqb200_clip_mse_workspace_bytes, 16-byte aligned)
+ * is private to the call.  FQB200_ERR_INVALID: a layout fqb200_clip_error does not take, K outside 1..256, prior not 0 or
+ * 1, a null x, stats, multipliers or out, bad num_bits / bit_alloc, max_ctas < 0; FQB200_ERR_WORKSPACE: a workspace that
+ * is missing, too small or misaligned.
+ */
+int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last, const float* stats,
+                    int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, int32_t prior,
+                    const float* multipliers, int32_t num_multipliers, double* out, float* out_params, void* workspace,
+                    size_t workspace_bytes, int32_t max_ctas, void* stream);
+/* Workspace of fqb200_clip_mse in bytes (0 and fqb200_last_error() on a layout or K it does not take). */
+size_t fqb200_clip_mse_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                                       int32_t num_multipliers);
+
+/*
  * 1-D k-means quantization of one weight tensor (pytorch_quantizer/quantization/kmeans_quantization.py:14-30): scikit-learn
  * 1.9's KMeans(n_clusters=k, random_state=seed).fit on the n floats of `in` in memory order (k = 2^num_bits, num_bits 1..8,
  * k <= n < 2^40): the data centred on its mean, one k-means++ init, Lloyd with max_iter 300 and tol = var(in) * 1e-4,
