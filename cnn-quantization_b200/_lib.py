@@ -73,6 +73,8 @@ PROTOTYPES = {
     "fqb200_clip_error_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32]),
     "fqb200_clip_mse": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _sz,
                                _i32, _vp]),
+    "fqb200_clip_mse_widths": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp,
+                                      _vp, _sz, _i32, _vp]),
     "fqb200_clip_mse_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
     "fqb200_kmeans1d": (_i32, [_vp, _i64, _i32, _i64, _vp, _i32, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
                                _i32, _vp]),

@@ -7,7 +7,10 @@
 //                 rule's b * F[bits]; then solve_range (alpha2DeltaOffset: float64 when solve_f64, else fp32) and
 //                 make_leaf_param(LEAF_TORCH) with the statistics of the [groups][FQB200_STATS_STRIDE] table of a stats_only
 //                 fqb200_fused launch on the same tensor (bits = that table's allocated width with bit_alloc), as
-//                 ce_candidate does for the three fixed candidates of fq_cliperr.cuh.
+//                 ce_candidate does for the three fixed candidates of fq_cliperr.cuh.  Prior 2 is the min/max range
+//                 (FQB200_RANGE_MINMAX, lower bound 0 when positive) and ignores m_k.
+//                 With per-candidate widths (`-bap mse`'s bit-allocation tables) candidate k quantizes at widths[k]
+//                 (0..8) instead, so one launch measures a channel's error at every width.
 //
 //   out[g] = { sum x^2,  sum (x - q_k)^2 (k = 0 .. K-1) }      d = x - q_k formed in float64 as in ce_add
 //
@@ -43,6 +46,8 @@ struct ClipMseArgs {
   const float* mult;                   // [K] clipping multipliers
   unsigned long long outer, groups, inner;
   int channels_last, num_bits, positive, bit_alloc, solve_f64, prior, K, Kpad;
+  int has_widths;                      // widths[k] is candidate k's width (else num_bits or the table's column 7)
+  unsigned char widths[kCmMaxK];
   unsigned long long units_per_group;  // NCHW: chunks of one group; channels-last: pixel chunks (of every slab)
   unsigned long long units;
   double* partial;                     // [groups][units_per_group][K + 1]
@@ -50,13 +55,15 @@ struct ClipMseArgs {
   float* params;                       // optional [groups][K][kCeParams]
 };
 
-// candidate k of group g: alpha = mult[k] * (b or std) - solve_range's k-std rule with the prior's scale in the std slot
+// candidate k of group g: alpha = mult[k] * (b or std) - solve_range's k-std rule with the prior's scale in the std slot -
+// or, prior 2, the min/max range
 __device__ __forceinline__ LeafParam cm_candidate(const ClipMseArgs& A, unsigned long long g, int k, float& delta, float& offset,
                                                   float& bits) {
   const float* t = A.stats + g * FQB200_STATS_STRIDE;
-  bits = A.bit_alloc ? __ldg(t + 7) : static_cast<float>(A.num_bits);
-  solve_range(FQB200_RANGE_KSTD, A.positive != 0, A.num_bits, __ldg(A.mult + k), A.solve_f64 != 0, __ldg(t + 0), __ldg(t + 1),
-              __ldg(t + 2), __ldg(t + 3), __ldg(t + (A.prior ? 4 : 3)), bits, delta, offset);
+  bits = A.has_widths ? static_cast<float>(A.widths[k]) : A.bit_alloc ? __ldg(t + 7) : static_cast<float>(A.num_bits);
+  solve_range(A.prior == 2 ? FQB200_RANGE_MINMAX : FQB200_RANGE_KSTD, A.positive != 0, A.num_bits, __ldg(A.mult + k),
+              A.solve_f64 != 0, __ldg(t + 0), __ldg(t + 1), __ldg(t + 2), __ldg(t + 3), __ldg(t + (A.prior ? 4 : 3)), bits,
+              delta, offset);
   return make_leaf_param(FQB200_LEAF_TORCH, delta, offset, bits);
 }
 
@@ -65,7 +72,7 @@ struct CmSmem {
   double* acc;                // [K + 1][S]: sum x^2, then the candidates' sums
   double* red;                // [2][kCmWarps][kCmTile][S]: fold buffers, alternating
   float *scale, *zp, *rcp;    // [Kpad][S]: the candidates' leaf parameters and reciprocals (Kpad - K copies of the last)
-  float* qmax;                // [S]
+  float* qmax;                // [S]; with per-candidate widths qmax = 2^w - 1 comes from the width instead
 };
 __host__ __device__ inline size_t cm_smem_bytes(int K, int S) {
   const int kpad = (K + kCmTile - 1) / kCmTile * kCmTile;
@@ -180,7 +187,7 @@ __device__ __forceinline__ void cm_unit(const ClipMseArgs& A, const CmSmem& sm, 
         const int i = (k0 + t) * S + slot;
         q[t].a = sm.scale[i];
         q[t].b = sm.zp[i];
-        q[t].c = qmax;
+        q[t].c = A.has_widths ? static_cast<float>((1 << A.widths[min(k0 + t, A.K - 1)]) - 1) : qmax;
         q[t].flags = FLAG_TRUE_ZERO;
         dv[t].s = q[t].a;
         dv[t].r = sm.rcp[i];

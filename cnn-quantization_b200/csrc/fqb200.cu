@@ -2651,13 +2651,31 @@ int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inne
                     int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, int32_t prior,
                     const float* multipliers, int32_t num_multipliers, double* out, float* out_params, void* workspace,
                     size_t workspace_bytes, int32_t max_ctas, void* stream) {
+  return fqb200_clip_mse_widths(in, outer, groups, inner, channels_last, stats, num_bits, positive, bit_alloc, solve_f64, prior,
+                                multipliers, nullptr, num_multipliers, out, out_params, workspace, workspace_bytes, max_ctas,
+                                stream);
+}
+
+int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                           int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
+                           double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
+                           void* stream) {
   g_err[0] = 0;
   const char* bad = clipmse_bad_args(outer, groups, inner, channels_last, num_multipliers);
   if (bad) return fail(FQB200_ERR_INVALID, bad);
   if (!in || !stats || !multipliers || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
   if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
   if (bit_alloc && num_bits > 4) return fail(FQB200_ERR_INVALID, "bit_alloc applies to num_bits <= 4 only%s");
-  if (prior != 0 && prior != 1) return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b) or 1 (Gauss std)%s");
+  if (widths) {
+    if (prior < 0 || prior > 2) return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b), 1 (Gauss std) or 2 (min/max)%s");
+    if (bit_alloc) return fail(FQB200_ERR_INVALID, "widths and bit_alloc are two sources of widths: pass one%s");
+    for (int k = 0; k < num_multipliers; ++k)
+      if (widths[k] < 0 || widths[k] > 8) return fail(FQB200_ERR_INVALID, "widths must be in 0..8%s");
+  } else {
+    if (prior == 2) return fail(FQB200_ERR_INVALID, "prior 2 (min/max) ignores the multipliers: it needs widths%s");
+    if (prior != 0 && prior != 1) return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b) or 1 (Gauss std)%s");
+  }
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
   int rc = check_workspace(workspace, workspace_bytes, clipmse_workspace(outer, groups, inner, channels_last, num_multipliers),
                            "fqb200_clip_mse_workspace_bytes");
@@ -2682,6 +2700,8 @@ int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inne
   A.prior = prior;
   A.K = num_multipliers;
   A.Kpad = (num_multipliers + fqb::kCmTile - 1) / fqb::kCmTile * fqb::kCmTile;
+  A.has_widths = widths ? 1 : 0;
+  for (int k = 0; widths && k < num_multipliers; ++k) A.widths[k] = static_cast<unsigned char>(widths[k]);
   A.units_per_group = clipmse_units_per_group(outer, inner, channels_last);
   A.units = A.units_per_group * (channels_last ? (A.groups + fqb::kCmSlab - 1) / fqb::kCmSlab : A.groups);
   A.partial = static_cast<double*>(workspace);

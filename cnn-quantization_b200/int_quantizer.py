@@ -50,6 +50,12 @@ def _build_tables():
 
 omega_table, alpha_table = _build_tables()
 
+# ACIQ clipping factors per bit width (int_quantizer.py:74-77)
+ALPHA_GAUS = {1: 1.24, 2: 1.71, 3: 2.15, 4: 2.55, 5: 2.93, 6: 3.28, 7: 3.61, 8: 3.92}
+ALPHA_GAUS_POSITIVE = {1: 1.71, 2: 2.15, 3: 2.55, 4: 2.93, 5: 3.28, 6: 3.61, 7: 3.92, 8: 4.2}
+ALPHA_LAPLACE = {0: 1.05, 1: 1.86, 2: 2.83, 3: 3.89, 4: 5.03, 5: 6.2, 6: 7.41, 7: 8.64, 8: 9.89}
+ALPHA_LAPLACE_POSITIVE = {0: 1.86, 1: 2.83, 2: 3.89, 3: 5.02, 4: 6.2, 5: 7.41, 6: 8.64, 7: 9.89, 8: 11.16}
+
 
 def _to_dev(t, device):
     if isinstance(t, torch.Tensor):
@@ -86,16 +92,18 @@ class IntQuantizer(object):
         self.measure_entropy = params["measure_entropy"]
         self.logger = params["logger"]
         self.mtd_quant = params["mtd_quant"]
-        self.alpha_gaus = {1: 1.24, 2: 1.71, 3: 2.15, 4: 2.55, 5: 2.93, 6: 3.28, 7: 3.61, 8: 3.92}
-        self.alpha_gaus_positive = {1: 1.71, 2: 2.15, 3: 2.55, 4: 2.93, 5: 3.28, 6: 3.61, 7: 3.92, 8: 4.2}
-        self.alpha_laplace = {0: 1.05, 1: 1.86, 2: 2.83, 3: 3.89, 4: 5.03, 5: 6.2, 6: 7.41, 7: 8.64, 8: 9.89}
-        self.alpha_laplace_positive = {0: 1.86, 1: 2.83, 2: 3.89, 3: 5.02, 4: 6.2, 5: 7.41, 6: 8.64, 7: 9.89, 8: 11.16}
+        self.alpha_gaus = dict(ALPHA_GAUS)
+        self.alpha_gaus_positive = dict(ALPHA_GAUS_POSITIVE)
+        self.alpha_laplace = dict(ALPHA_LAPLACE)
+        self.alpha_laplace_positive = dict(ALPHA_LAPLACE_POSITIVE)
         # statistics manager for `-sm use`: a zero-argument callable returning the manager (the reference stores the
         # singleton CLASS here, inference_quantization_manager.py:413,450,464,471; any object with
         # get_tensor_stat(id, stat, kind) works)
         self.sm = None
         # `-c mse`: the statistics.ClipMseStatistics that reads the collected clipping-MSE curves (set by the manager)
         self.mse_curves = None
+        # `-bap mse`: the statistics.BitMseStatistics that reads the collected per-channel error tables (set by the manager)
+        self.bit_tables = None
         self._stat_cache = {}  # offline-statistics parameters are constants of a layer: solved once, kept on the device
         self.force_positive = False
         self.half_range = False
@@ -255,6 +263,10 @@ class IntQuantizer(object):
         raise NotImplementedError("clipping %r needs offline statistics or is undefined in the reference" % clip_type)
 
     def _prior(self):
+        """The prior of the on-the-fly activation launches' bit allocation."""
+        if self.bit_alloc_prior == "mse" and self.bit_alloc_act:
+            raise NotImplementedError("-baa -bap mse allocates from per-channel error tables collected with collect_bits: "
+                                      "it needs -sm use")
         return L.PRIOR_STD if self.bit_alloc_prior == "gaus" else L.PRIOR_B
 
     @staticmethod
@@ -382,10 +394,33 @@ class IntQuantizer(object):
         return v
 
     def _stat_bits(self, stat_id, device, target):
-        """Per-channel bit widths from the collected prior statistic (int_quantizer.py:236-247, :430-438)."""
+        """Per-channel bit widths from the collected prior statistic (int_quantizer.py:236-247, :430-438), or with
+        ``bit_alloc_prior="mse"`` the widths bit_alloc.allocate gives the layer's collected error tables."""
+        if self.bit_alloc_prior == "mse":
+            return self._mse_bits(stat_id, device, target)
         prior = "std" if self.bit_alloc_prior == "gaus" else "b"
         pr = _to_dev(np.asarray(self._stat(stat_id, prior, "mean"), dtype=np.float32), device)
         return self.get_bits_alloc_fixed_target(pr, target, self.bit_alloc_round)
+
+    def _mse_bits(self, stat_id, device, target):
+        """`-bap mse`: float32 [C] widths minimising the sum of the layer's measured per-channel errors (bit_mse.pkl,
+        collected with collect_bits under this run's clipping rule) for the budget of ``target`` bits per channel."""
+        from .bit_alloc import allocate
+        if self.kld or self.clipping not in ("laplace", "gaus", "no"):
+            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus or no, not %s"
+                                      % ("-kld" if self.kld else "-c " + self.clipping))
+        if self.bit_tables is None:
+            raise KeyError("-bap mse needs the per-channel error tables of layer %r: collect them with collect_bits=True"
+                           % (stat_id,))
+        mse, rule = self.bit_tables.table(stat_id)
+        if rule != self.clipping:
+            raise ValueError("-bap mse: the tables of %r were measured under -c %s, this run clips with -c %s"
+                             % (stat_id, rule, self.clipping))
+        channels = np.size(self._stat(stat_id, "max", "mean"))
+        if mse.shape[0] != channels:
+            raise ValueError("-bap mse: the table of %r has %d groups, the statistics %d channels"
+                             % (stat_id, mse.shape[0], channels))
+        return torch.tensor(allocate(mse, target), dtype=torch.float32, device=device)
 
     def _clipping_params_from_stats(self, tensor, stat_id, clip_type):
         """(delta, offset, bits, per_channel) of gemmlowpClippingQuantize in use mode (int_quantizer.py:327-359 with
@@ -651,15 +686,46 @@ class IntQuantizer(object):
             mx = _to_dev(max_, tensor.device) if max_ is not None else t.max(-1)[0]
             bits = None
             if self.bit_alloc_weight and self.num_bits <= 4:
+                if self.bit_alloc_prior == "mse":
+                    raise NotImplementedError("-baw -bap mse measures the weight's own min/max range: explicit min_ / max_ "
+                                              "bounds are not supported")
                 bits = self.get_bits_alloc_fixed_target(t.std(-1), self.bit_alloc_target_weight, self.bit_alloc_round)
             return ops.quantize1(tensor, mx - mn, mn, self.num_bits, bits=bits, layout=layout)
         bc, vc = weight_correction if weight_correction is not None else (False, False)
+        if self.bit_alloc_weight and self.num_bits <= 4 and self.bit_alloc_prior == "mse":
+            return self._mse_weights(tensor, id, layout, bc, vc)
         hist = self._hist(tensor)
         res = self._fused(tensor, layout, scope=L.SCOPE_GROUP, range_mode=L.RANGE_MINMAX, leaf=L.LEAF_TORCH,
                         num_bits=self.num_bits, positive=False, bit_alloc=self.bit_alloc_weight,
                         bit_alloc_prior=L.PRIOR_STD, bit_alloc_round=self.bit_alloc_round,
                         bit_alloc_target=self.bit_alloc_target_weight, bias_corr=bc, var_corr=vc, hist=hist)
         self._log_entropy(hist, id, "avg.entropy.weight", tensor.numel())
+        return res
+
+    def _mse_weights(self, tensor, id, layout, bias_corr, var_corr):
+        """`-baw -bap mse`: per output channel the min/max range, at the widths that minimise the weight's measured
+        squared error for the budget of bit_alloc_target_weight bits per channel: a statistics-only launch, one
+        ops.clip_mse over widths 0..8, bit_alloc.allocate on the host, then one given-parameter launch (with `-me`, its
+        grid gives the entropy).  The bias and variance corrections follow as stock torch ops on the NCHW-ordered weight
+        (a channels-last weight is read in that order by every launch here, and the result comes back in it)."""
+        from .bit_alloc import MAX_BITS, allocate
+        table = ops.fused(tensor, layout, num_bits=8, stats_only=True)
+        widths = list(range(MAX_BITS + 1))
+        sse = ops.clip_mse(tensor, table, layout, False, self.num_bits, False, [0.0] * len(widths), prior="minmax",
+                           widths=widths, solve_f64=False)
+        bits = torch.tensor(allocate(sse[:, 1:], self.bit_alloc_target_weight), dtype=torch.float32, device=tensor.device)
+        mn, mx = table[:, 0].contiguous(), table[:, 1]
+        if self.measure_entropy:
+            res, grid = ops.quantize1(tensor, (mx - mn).contiguous(), mn, self.num_bits, bits=bits, layout=layout,
+                                      want_grid=True)
+            hist = torch.bincount(grid.flatten().to(torch.int64).clamp_(0, 255), minlength=256)
+            self._log_entropy(hist, id, "avg.entropy.weight", tensor.numel())
+        else:
+            res = ops.quantize1(tensor, (mx - mn).contiguous(), mn, self.num_bits, bits=bits, layout=layout)
+        if bias_corr or var_corr:
+            from .manager import QuantizationManagerInference
+            res = QuantizationManagerInference._weight_correction_torch(tensor.contiguous(), res.contiguous(), bias_corr,
+                                                                        var_corr)
         return res
 
     # mid-tread "bin allocation" quantizer, int_quantizer.py:147-225
@@ -710,7 +776,12 @@ class IntQuantizer(object):
         if self.logger is not None:
             self.logger.log_metric(id + ".entropy", entropy.item(), step="auto", meterId=meter, weight=numel)
 
+    def _mid_tread_bins(self):
+        if self.bit_alloc_prior == "mse":
+            raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
+
     def mid_tread_quantize_weights_per_channel(self, tensor, id, weight_correction=None):
+        self._mid_tread_bins()
         rows = tensor.shape[0]
         bc, vc = weight_correction if weight_correction is not None else (False, False)
         if self.measure_entropy:
@@ -720,6 +791,7 @@ class IntQuantizer(object):
                          mt_target=self.bit_alloc_target_weight, mt_clip=False, bias_corr=bc, var_corr=vc)
 
     def mid_tread_quantize_activation(self, tensor, id, bias=None):
+        self._mid_tread_bins()
         if self._pc_act(tensor):
             return self.mid_tread_quantize_activation_per_channel(tensor, id, bias=bias)
         if bias is not None:
@@ -728,6 +800,7 @@ class IntQuantizer(object):
                          mt_target=self.bit_alloc_target_act, mt_clip=True, out=self._out(tensor))
 
     def mid_tread_quantize_activation_per_channel(self, tensor, id, bias=None):
+        self._mid_tread_bins()
         layout = self._nchw_layout(tensor)
         kw = dict(leaf=L.LEAF_MIDTREAD, positive=self._positive(), mt_target=self.bit_alloc_target_act, mt_clip=True, bias=bias,
                   out=self._out(tensor), channels_last=ops.cl_eligible(tensor))
@@ -749,6 +822,7 @@ class IntQuantizer(object):
 
     def mid_tread_quantization(self, tensor, id, target, clip=False, sym=True):
         """[R, K] view, int_quantizer.py:185-225.  Returns (quantized, None) like the reference without entropy."""
+        self._mid_tread_bins()
         out = self._fused(tensor, (1, tensor.shape[0], tensor.numel() // tensor.shape[0]), leaf=L.LEAF_MIDTREAD,
                         positive=not sym, mt_target=target, mt_clip=clip)
         return out, None
@@ -844,6 +918,9 @@ class IntQuantizer(object):
     def get_alpha_laplace(self, tensor, stat_id=None, kind="mean", per_channel=False):
         """int_quantizer.py:227-253."""
         self._unsupported(stat_id)
+        if self.bit_alloc_act and per_channel and self.num_bits <= 4 and self.bit_alloc_prior == "mse":
+            raise NotImplementedError("-baa -bap mse allocates from per-channel error tables collected with collect_bits: "
+                                      "it needs -sm use")
         stats = self.__act_stats_perchannel__ if per_channel else self.__act_stats__
         b = stats(tensor, ["b"])["b"]
         table = self.alpha_laplace_positive if self._positive() else self.alpha_laplace

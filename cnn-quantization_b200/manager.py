@@ -35,7 +35,10 @@ def make_args(**over):
     mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument), ``collect_mse`` (also
     write the clipping-MSE curve of every call site's quantizer in `-sm collect`, over ``mse_multipliers`` - default
     statistics.MSE_MULTIPLIERS, 0.5 .. 16 in steps of 0.125 - times the Laplace b or, with ``mse_prior="gaus"``, the std;
-    `-c mse` in use mode clips at the minimum of those curves) and
+    `-c mse` in use mode clips at the minimum of those curves), ``collect_bits`` (also write, for every call site `-sm use`
+    quantizes per channel with bit allocation, the error of its quantizer on each channel at every width 0..8; needs
+    ``per_channel_quant_act``, ``bit_alloc_act`` and clipping laplace, gaus or no; ``bit_alloc_prior="mse"`` (`-bap mse`) then allocates the
+    widths that minimise the sum of those errors, and allocates weight widths from the weights' own errors) and
     ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms; "angle", the
     pairwise sample angles of its angle_stats module, which the reference selects by editing an import; or "noise", the
     per-sample quantization error statistics of its measure_statistics module, which the reference cannot run)."""
@@ -45,7 +48,8 @@ def make_args(**over):
              bit_alloc_rmode="round", bit_alloc_prior="gaus", bit_alloc_target_act=None, bit_alloc_target_weight=None,
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
              mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
-             collect_err=False, measure_stats_kind="distance", collect_mse=False, mse_multipliers=None, mse_prior="laplace")
+             collect_err=False, measure_stats_kind="distance", collect_mse=False, mse_multipliers=None, mse_prior="laplace",
+             collect_bits=False)
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -413,6 +417,31 @@ class QuantizationManagerInference(object):
             raise ValueError("collect_mse measures the clipping-MSE curves of -sm collect for the bit widths of -qtype: it "
                              "needs stats_mode='collect' and a qtype (got stats_mode=%r, qtype=%r)" % (self.stats_mode, args.qtype))
         self.clip_mse = None
+        # `collect_bits`: the collect hooks also measure the per-channel error tables `-bap mse` allocates from
+        self.collect_bits = bool(getattr(args, "collect_bits", False))
+        if self.collect_bits:
+            missing = [what for what, ok in (("stats_mode='collect'", self.stats_mode == "collect"),
+                                              ("a qtype", args.qtype is not None),
+                                              ("per_channel_quant_act", args.per_channel_quant_act),
+                                              ("bit_alloc_act", args.bit_alloc_act),
+                                              ("clipping laplace, gaus or no", args.clipping in ("laplace", "gaus", "no")))
+                       if not ok]
+            if missing:
+                raise ValueError("collect_bits measures the per-channel error tables of -sm collect: it needs %s"
+                                 % ", ".join(missing))
+        bap_mse = getattr(args, "bit_alloc_prior", None) == "mse"
+        if bap_mse and (args.kld_threshold or args.clipping in ("mix", "mse")):
+            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus or no, not %s"
+                                      % ("-kld" if args.kld_threshold else "-c " + args.clipping))
+        if bap_mse and getattr(args, "mid_thread_quant", False):
+            raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
+        if bap_mse and args.bit_alloc_act and self.stats_mode == "no":
+            raise NotImplementedError("-baa -bap mse allocates from collected tables: it needs -sm use (collect them with "
+                                      "collect_bits=True)")
+        if bap_mse and args.bit_alloc_act and (self.collect_err or self.collect_mse):
+            raise NotImplementedError("-baa -bap mse: collect_err and collect_mse would measure their candidates at the "
+                                      "analytic widths, not at the widths -bap mse runs with")
+        self.bit_mse = None
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None
         self._sm_tensor = self._sm_channel = None
@@ -434,6 +463,9 @@ class QuantizationManagerInference(object):
                     from .statistics import ClipMseStatistics
                     self.clip_mse = ClipMseStatistics(sf, getattr(args, "mse_multipliers", None),
                                                       getattr(args, "mse_prior", "laplace"), base_dir=base)
+                if self.collect_bits:
+                    from .statistics import BitMseStatistics
+                    self.bit_mse = BitMseStatistics(sf, args.clipping, base_dir=base)
             else:
                 if args.per_channel_quant_act:
                     self._sm_channel = StatisticManagerPerChannel(sf, load_stats=True, base_dir=base)
@@ -441,6 +473,9 @@ class QuantizationManagerInference(object):
                 if args.clipping == "mse":   # read on first use: a missing file raises KeyError naming collect_mse there
                     from .statistics import ClipMseStatistics
                     self.clip_mse = ClipMseStatistics(sf, base_dir=base, load=True)
+                if bap_mse:   # read on first use: a missing file raises KeyError naming collect_bits there
+                    from .statistics import BitMseStatistics
+                    self.bit_mse = BitMseStatistics(sf, base_dir=base, load=True)
         self.fused_relu = args.arch is not None and (args.arch in FUSED_RELU_ARCHS or "squeezenet" in args.arch)
         self.ignore_ids = []
         self.quantizers = {}
@@ -465,6 +500,7 @@ class QuantizationManagerInference(object):
                         continue
                     q.sm = per_channel if tag in ("activation", "weight", "weight_classifier", "") else per_tensor
                     q.mse_curves = self.clip_mse
+                    q.bit_tables = self.bit_mse
             if self.inplace_activations:
                 for tag, q in list(self.quantizers.items()) + [("", self.quantizer_default)]:
                     if tag.startswith("activation") or tag in ("", "ignored"):
@@ -562,6 +598,8 @@ class QuantizationManagerInference(object):
             self.stats_manager.__exit__()  # collect mode: write the CSV / pickle files
         if self.clip_mse is not None:
             self.clip_mse.__exit__()       # collect_mse: clip_mse.pkl and curve.csv
+        if self.bit_mse is not None:
+            self.bit_mse.__exit__()        # collect_bits: bit_mse.pkl and alloc.csv
         if self.measure_stats is not None:
             self.measure_stats.__exit__()  # -ms: write distance.csv (angle.pkl, noise/<id>.csv with the other kinds)
 
@@ -700,8 +738,9 @@ class QuantizationManagerInference(object):
         quantize_instant picks for the same call in `-sm use` (``tag``, the 8-bit ``ignored`` list, ``half_range``) on
         this tensor ``out``: per channel when it would quantize it per channel, with bit allocation only then.  With
         collect_mse, the call site's clipping-MSE curve is measured here, with the same settings (``name``: the
-        internal name save_tensor_stats records)."""
-        if not (self.collect_err or self.collect_mse):
+        internal name save_tensor_stats records).  With collect_bits, a call site it would quantize per channel with bit
+        allocation also gets its per-channel error tables measured."""
+        if not (self.collect_err or self.collect_mse or self.collect_bits):
             return {}
         from .statistics import ClipErrConfig
         q = self.get_quantizer("ignored" if stat_id in self.ignore_ids else tag)
@@ -712,6 +751,8 @@ class QuantizationManagerInference(object):
                             bit_alloc_round=bool(q.bit_alloc_round), bit_alloc_target=q.bit_alloc_target_act)
         if self.collect_mse:
             self.clip_mse.save_curve(out, name, stat_id, cfg)
+        if self.collect_bits:
+            self.bit_mse.save_table(out, name, stat_id, cfg)
         return {"clip_err": cfg} if self.collect_err else {}
 
     def _stat_id(self, activation_id):

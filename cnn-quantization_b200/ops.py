@@ -621,25 +621,27 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
     return (out, params) if want_params else out
 
 
-CLIP_MSE_PRIORS = {"laplace": 0, "gaus": 1}
+CLIP_MSE_PRIORS = {"laplace": 0, "gaus": 1, "minmax": 2}
 
 
 def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, prior="laplace", bit_alloc=False,
-             solve_f64=None, want_params=False, max_ctas=0):
+             solve_f64=None, want_params=False, max_ctas=0, widths=None):
     """C ABI fqb200_clip_mse: per group of ``layout`` = (outer, groups, inner), the clipping-MSE curve of the quantizer
     ``clip_error`` describes, over K = len(``multipliers``) (1..256) clipping values alpha_k = multipliers[k] * b
     (``prior`` "laplace") or * std ("gaus"), as a [groups, K + 1] float64 device tensor: column 0 sum x^2, column 1 + k
     sum (x - q_k)^2.  ``table``, ``channels_last``, ``bit_alloc`` and ``solve_f64`` as in ``clip_error``; a multiplier equal
     to the ACIQ Laplace factor of the width gives its Laplace candidate.  ``multipliers``: a sequence of floats or a
-    float32 tensor (rounded to float32).  Deterministic, no host synchronisation; with ``want_params`` also returns the
-    [groups, K, 6] candidate parameters (delta, offset, bits, scale, zero point, qmax).  Recorded in the launch profile
-    under mode 'R' (one read of the tensor)."""
+    float32 tensor (rounded to float32).  ``widths`` (fqb200_clip_mse_widths): K ints in 0..8, candidate k's bit width
+    instead of ``num_bits`` (not with ``bit_alloc``); only then ``prior`` may also be "minmax", the table's min/max range
+    (0 as the lower bound when ``positive``), which ignores the multipliers.  Deterministic, no host synchronisation; with
+    ``want_params`` also returns the [groups, K, 6] candidate parameters (delta, offset, bits, scale, zero point, qmax).
+    Recorded in the launch profile under mode 'R' (one read of the tensor)."""
     _require_cuda_f32(x, "tensor")
     outer, groups, inner = (int(v) for v in layout)
     if outer * groups * inner != x.numel():
         raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
-    if prior not in CLIP_MSE_PRIORS:
-        raise ValueError("prior must be one of %s, got %r" % (sorted(CLIP_MSE_PRIORS), prior))
+    if prior not in CLIP_MSE_PRIORS or (prior == "minmax" and widths is None):
+        raise ValueError("prior must be one of %s (minmax with widths only), got %r" % (sorted(CLIP_MSE_PRIORS), prior))
     if channels_last:
         if not cl_eligible(x, layout):
             raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
@@ -653,6 +655,10 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
     k = mult.numel()
     if not 1 <= k <= 256:
         raise ValueError("clip_mse takes 1..256 multipliers, got %d" % k)
+    if widths is not None:
+        widths = np.ascontiguousarray(widths, dtype=np.int32).reshape(-1)   # host values, validated by the library
+        if widths.size != k:
+            raise ValueError("clip_mse: %d widths for %d multipliers" % (widths.size, k))
     lib = L.load()
     dev = x.device
     if solve_f64 is None:
@@ -663,10 +669,14 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
         out.zero_()
         return (out, params) if want_params else out
     ws = _own_workspace(dev, lib.fqb200_clip_mse_workspace_bytes(outer, groups, inner, int(bool(channels_last)), k))
-    _launch(dev, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse, x.data_ptr(), outer,
-            groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), int(bool(bit_alloc)),
-            int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), k, out.data_ptr(), _ptr(params), ws.data_ptr(),
-            ws.numel(), int(max_ctas))
+    head = (x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)),
+            int(bool(bit_alloc)), int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr())
+    tail = (k, out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
+    timed = _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner))
+    if widths is None:
+        _launch(dev, timed, lib.fqb200_clip_mse, *head, *tail)
+    else:
+        _launch(dev, timed, lib.fqb200_clip_mse_widths, *head, widths.ctypes.data, *tail)
     return (out, params) if want_params else out
 
 

@@ -51,6 +51,17 @@ reads back in use mode:
 
 Each hooked tensor costs one statistics-only launch and one ops.clip_mse launch pair; the sums stay on the device until
 ``__exit__``, which reads everything back in one copy.
+
+``BitMseStatistics`` is the per-channel error table of every collect call site that `-sm use` quantizes per channel with
+bit allocation (`collect_bits`): the error the call site's quantizer makes on each channel at every width 0..8, and what
+`-bap mse` allocates from in use mode:
+
+    <base>/bit_mse/<folder>/bit_mse.pkl     {"rule", id: DataFrame[count, b, std, positive, mse_w0 .. mse_w8], one row
+                                            per channel}
+    <base>/bit_mse/<folder>/alloc.csv       id, internal_name, groups, target, and bits_* / mse_* (bit sum, per-element
+                                            MSE) of the uniform width, the analytic allocation and the measured one
+
+It costs the same as ``ClipMseStatistics`` with 9 candidates.
 """
 import collections
 import os
@@ -64,7 +75,7 @@ import torch
 from . import ops
 
 __all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "AngleStatistics", "NoiseStatistics",
-           "ClipErrConfig", "ClipMseStatistics", "MSE_MULTIPLIERS", "default_base_dir"]
+           "ClipErrConfig", "ClipMseStatistics", "MSE_MULTIPLIERS", "BitMseStatistics", "bit_candidates", "default_base_dir"]
 
 
 def default_base_dir():
@@ -580,8 +591,8 @@ class ClipMseStatistics(object):
     range, the relation the reference's *_positive ACIQ tables encode), weighted by the group's count."""
 
     def __init__(self, folder, multipliers=None, prior="laplace", base_dir=None, load=False):
-        if prior not in ops.CLIP_MSE_PRIORS:
-            raise ValueError("mse_prior must be one of %s, got %r" % (sorted(ops.CLIP_MSE_PRIORS), prior))
+        if prior not in ("gaus", "laplace"):
+            raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
         self.folder = os.path.join(base_dir or default_base_dir(), "clip_mse", folder)
         self.multipliers = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers, dtype=np.float32).reshape(-1)
         if not 1 <= self.multipliers.size <= 256:
@@ -687,3 +698,130 @@ class ClipMseStatistics(object):
             raise KeyError("-c mse needs the clipping-MSE curve of layer %r: collect it with collect_mse=True" % (id,))
         m = self.curves["multipliers"]
         return best_multipliers(m, df[["mse_%d" % j for j in range(len(m))]].to_numpy()), self.curves["prior"]
+
+
+BIT_RULES = ("laplace", "gaus", "no")
+
+
+def bit_candidates(rule, positive, num_bits):
+    """(multipliers, ops.clip_mse prior) of the 9 candidates of width w = 0..8: what `-sm use` runs on a channel
+    allocated w bits under the clipping ``rule`` - the Laplace ACIQ factor of w on b (int_quantizer.py:236-253), the Gauss
+    factor of ``num_bits`` on std for every width (:264), or the min/max range (:409-451, :453-476)."""
+    from .int_quantizer import ALPHA_GAUS, ALPHA_GAUS_POSITIVE, ALPHA_LAPLACE, ALPHA_LAPLACE_POSITIVE
+    widths = range(9)
+    if rule == "laplace":
+        table = ALPHA_LAPLACE_POSITIVE if positive else ALPHA_LAPLACE
+        return [table[w] for w in widths], "laplace"
+    if rule == "gaus":
+        return [(ALPHA_GAUS_POSITIVE if positive else ALPHA_GAUS)[num_bits]] * 9, "gaus"
+    if rule == "no":
+        return [0.0] * 9, "minmax"
+    raise ValueError("bit allocation tables are measured under clipping %s, got %r" % (list(BIT_RULES), rule))
+
+
+class BitMseStatistics(object):
+    """Per-channel error tables of bit allocation (`collect_bits`): ``save_table(t, tag, id, cfg)`` adds, for a call site
+    whose quantizer ``cfg`` (a ClipErrConfig) quantizes per channel with bit allocation, the float64 sums of one
+    ops.clip_mse launch over the 9 candidates of ``bit_candidates(rule, ...)`` and the channels' b and std to device
+    accumulators; other call sites are skipped.  ``__exit__`` writes bit_mse.pkl and alloc.csv.  With ``load`` the instance
+    reads bit_mse.pkl instead (on first use), for `-bap mse`."""
+
+    def __init__(self, folder, rule=None, base_dir=None, load=False):
+        if not load and rule not in BIT_RULES:
+            raise ValueError("collect_bits measures under clipping %s, got %r" % (list(BIT_RULES), rule))
+        self.folder = os.path.join(base_dir or default_base_dir(), "bit_mse", folder)
+        self.rule = rule
+        self.load = load
+        self.tables = None
+        self.acc = {}    # id -> (sums [G, 10], b / std sums [G, 2], float64 device tensors, batches)
+        self.meta = {}   # id -> (internal_name, ClipErrConfig, elements per channel and batch)
+        self._mult_dev = {}
+
+    # -- collect ---------------------------------------------------------------------------------------------------
+    def save_table(self, tensor, tag, id, cfg):
+        if not (cfg.per_channel and cfg.bit_alloc):
+            return
+        t = tensor.detach()
+        n, c = t.shape[0], t.shape[1]
+        layout = (n, c, t.numel() // (n * c))
+        cl = ops.cl_eligible(t, layout)
+        if not cl:
+            t = t.contiguous()
+        table = ops.fused(t, layout, num_bits=8, stats_only=True, channels_last=cl)
+        mults, prior = bit_candidates(self.rule, cfg.positive, cfg.num_bits)
+        key = (t.device, bool(cfg.positive), cfg.num_bits)
+        mult = self._mult_dev.get(key)
+        if mult is None:
+            mult = self._mult_dev[key] = torch.tensor(mults, dtype=torch.float32, device=t.device)
+        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=prior, widths=range(9),
+                            solve_f64=False)
+        scales = table[:, 3:5].double()
+        prev = self.acc.get(id)
+        if prev is None:
+            self.acc[id] = (sums, scales, 1)
+            self.meta[id] = (tag, cfg, layout[0] * layout[2])
+        else:
+            if prev[0].shape != sums.shape:
+                raise ValueError("collect_bits of %r: %d channels in this call, %d before" % (id, sums.shape[0], prev[0].shape[0]))
+            self.acc[id] = (prev[0] + sums, prev[1] + scales, prev[2] + 1)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *args):
+        if self.load or not self.acc:
+            return
+        import pandas as pd
+        from . import _lib as L
+        from .bit_alloc import allocate
+        from .int_quantizer import IntQuantizer
+        flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
+        out = {"rule": self.rule}
+        rows = []
+        pos = 0
+        for id in list(self.acc):
+            sums, _, batches = self.acc[id]
+            g = sums.shape[0]
+            s = flat[pos:pos + g * 10].reshape(g, 10)
+            pos += g * 10
+            sc = flat[pos:pos + g * 2].reshape(g, 2) / batches
+            pos += g * 2
+            tag, cfg, per_batch = self.meta[id]
+            count = np.full(g, float(per_batch * batches))
+            mse = s[:, 1:] / count[:, None]
+            df = pd.DataFrame({"count": count, "b": sc[:, 0], "std": sc[:, 1], "positive": np.full(g, bool(cfg.positive))})
+            out[id] = pd.concat([df, pd.DataFrame(mse, columns=["mse_w%d" % w for w in range(9)])], axis=1)
+            prior = sc[:, 0] if cfg.bit_alloc_prior == L.PRIOR_B else sc[:, 1]
+            analytic = IntQuantizer.get_bits_alloc_fixed_target(torch.from_numpy(prior.astype(np.float32)),
+                                                                cfg.bit_alloc_target, cfg.bit_alloc_round)
+            allocations = (np.full(g, cfg.num_bits), analytic.numpy().astype(np.int64), allocate(mse, cfg.bit_alloc_target))
+            row = [id, tag, g, cfg.bit_alloc_target]
+            for w in allocations:
+                row += [int(w.sum()), float(s[np.arange(g), 1 + w].sum() / count.sum())]
+            rows.append(row)
+        if os.path.exists(self.folder):
+            shutil.rmtree(self.folder)
+        os.makedirs(self.folder)
+        with open(os.path.join(self.folder, "bit_mse.pkl"), "wb") as f:
+            pickle.dump(out, f)
+        pd.DataFrame(rows, columns=ALLOC_COLUMNS).to_csv(os.path.join(self.folder, "alloc.csv"), index=False)
+        self.acc, self.meta = {}, {}
+
+    # -- use (`-bap mse`) --------------------------------------------------------------------------------------------
+    def table(self, id):
+        """(float64 [C, 9] per-element MSE of widths 0..8, rule) collected for ``id``; KeyError naming collect_bits when
+        there is none."""
+        if self.tables is None:
+            path = os.path.join(self.folder, "bit_mse.pkl")
+            if not os.path.exists(path):
+                raise KeyError("-bap mse needs the per-channel error tables at %s: collect them with collect_bits=True" % path)
+            with open(path, "rb") as f:
+                self.tables = pickle.load(f)
+        df = self.tables.get(id)
+        if df is None:
+            raise KeyError("-bap mse needs the per-channel error table of layer %r: collect it with collect_bits=True" % (id,))
+        return df[["mse_w%d" % w for w in range(9)]].to_numpy(dtype=np.float64), self.tables["rule"]
+
+
+ALLOC_COLUMNS = ["id", "internal_name", "groups", "target", "bits_uniform", "mse_uniform", "bits_analytic", "mse_analytic",
+                 "bits_measured", "mse_measured"]

@@ -390,7 +390,21 @@ int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inne
                     int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64, int32_t prior,
                     const float* multipliers, int32_t num_multipliers, double* out, float* out_params, void* workspace,
                     size_t workspace_bytes, int32_t max_ctas, void* stream);
-/* Workspace of fqb200_clip_mse in bytes (0 and fqb200_last_error() on a layout or K it does not take). */
+/*
+ * fqb200_clip_mse with a bit width per candidate (the per-channel error tables of `-bap mse`): candidate k quantizes at
+ * widths[k] instead of num_bits, everything else as fqb200_clip_mse.  `widths` is a host array of K values in 0..8 (read
+ * before the call returns; width 0 is the torch leaf with qmax 0); NULL is fqb200_clip_mse.  With widths, prior 2 is the
+ * min/max range (FQB200_RANGE_MINMAX from the table's min and max, 0 as the lower bound when `positive`), which ignores
+ * the multipliers.  The workspace is fqb200_clip_mse_workspace_bytes.  FQB200_ERR_INVALID, before any CUDA call, also on:
+ * a width outside 0..8, widths together with bit_alloc (two sources of widths), prior 2 without widths, prior outside 0..2.
+ */
+int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                           int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
+                           double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
+                           void* stream);
+/* Workspace of fqb200_clip_mse and fqb200_clip_mse_widths in bytes (0 and fqb200_last_error() on a layout or K it does not
+ * take). */
 size_t fqb200_clip_mse_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                                        int32_t num_multipliers);
 
