@@ -76,6 +76,9 @@ PROTOTYPES = {
     "fqb200_clip_mse_widths": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp,
                                       _vp, _sz, _i32, _vp]),
     "fqb200_clip_mse_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
+    "fqb200_clip_mse_grid": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _i32, _vp,
+                                    _vp, _vp, _sz, _i32, _vp]),
+    "fqb200_clip_mse_grid_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32, _i32]),
     "fqb200_kmeans1d": (_i32, [_vp, _i64, _i32, _i64, _vp, _i32, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
                                _i32, _vp]),
     "fqb200_kmeans1d_workspace_bytes": (_sz, [_i64, _i32]),

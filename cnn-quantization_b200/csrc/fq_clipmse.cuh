@@ -11,18 +11,23 @@
 //                 (FQB200_RANGE_MINMAX, lower bound 0 when positive) and ignores m_k.
 //                 With per-candidate widths (`-bap mse`'s bit-allocation tables) candidate k quantizes at widths[k]
 //                 (0..8) instead, so one launch measures a channel's error at every width.
+//   grid launch   (fqb200_clip_mse_grid, the joint width-and-clip tables of `-c mse -bap mse`): nw widths times K
+//                 multipliers; candidate j = i * K + k quantizes at widths[i] and clips at mult[k].  The width is one
+//                 more unit dimension, so a unit runs one width's K candidates with one qmax, in the shared memory of a
+//                 K-candidate launch, and every column has the bits of the per-candidate-width launch on that pair.
 //
-//   out[g] = { sum x^2,  sum (x - q_k)^2 (k = 0 .. K-1) }      d = x - q_k formed in float64 as in ce_add
+//   out[g] = { sum x^2,  sum (x - q_j)^2 (j = 0 .. nw*K-1) }      d = x - q_j formed in float64 as in ce_add
 //
 //   fq_clipmse_partial_kernel  fixed work units: (group, chunk of kCmChunk elements) on NCHW / per-tensor layouts (128-bit
 //                              loads when inner % 4 == 0 and x is 16-byte aligned), (32-channel slab, kCmClRows pixels) on
-//                              channels-last [N][HW][C] memory (one channel per lane).  A unit first solves its candidates'
+//                              channels-last [N][HW][C] memory (one channel per lane), times the nw widths of a grid
+//                              launch (adjacent units, so the chunk's other reads hit L2).  A unit first solves its candidates'
 //                              parameters and divisors into shared memory.  It then walks its chunk in pieces of kCmPer
 //                              elements per thread, each loaded once from global memory into registers; every candidate
 //                              tile of kCmTile float64 accumulators runs over the piece in registers, and a fixed
 //                              warp / CTA tree adds the tile into the unit's shared-memory sums.  Each unit writes its own
-//                              workspace slot.
-//   fq_clipmse_finish_kernel   one CTA per group: adds the group's unit partials in unit order, writes out[g] and,
+//                              workspace slot; sum x^2 comes from the units of width 0 only.
+//   fq_clipmse_finish_kernel   one CTA per group: adds the group's unit partials in chunk order, writes out[g] and,
 //                              optionally, the candidates' parameters.
 //
 // No atomics touch the values: the result has the same bits on every run and for every grid size.  NaN propagates.
@@ -47,20 +52,25 @@ struct ClipMseArgs {
   unsigned long long outer, groups, inner;
   int channels_last, num_bits, positive, bit_alloc, solve_f64, prior, K, Kpad;
   int has_widths;                      // widths[k] is candidate k's width (else num_bits or the table's column 7)
+  int grid;                            // grid launch: widths[i] is the width of unit width index i (has_widths is 0)
+  int nw;                              // widths per (group, chunk): nw of a grid launch, else 1
   unsigned char widths[kCmMaxK];
   unsigned long long units_per_group;  // NCHW: chunks of one group; channels-last: pixel chunks (of every slab)
   unsigned long long units;
-  double* partial;                     // [groups][units_per_group][K + 1]
-  double* out;                         // [groups][K + 1]
-  float* params;                       // optional [groups][K][kCeParams]
+  double* partial;                     // [groups][units_per_group][nw * K + 1]
+  double* out;                         // [groups][nw * K + 1]
+  float* params;                       // optional [groups][nw * K][kCeParams]
 };
 
-// candidate k of group g: alpha = mult[k] * (b or std) - solve_range's k-std rule with the prior's scale in the std slot -
-// or, prior 2, the min/max range
-__device__ __forceinline__ LeafParam cm_candidate(const ClipMseArgs& A, unsigned long long g, int k, float& delta, float& offset,
-                                                  float& bits) {
+// candidate k (of width index wi in a grid launch) of group g: alpha = mult[k] * (b or std) - solve_range's k-std rule
+// with the prior's scale in the std slot - or, prior 2, the min/max range
+__device__ __forceinline__ LeafParam cm_candidate(const ClipMseArgs& A, unsigned long long g, int k, int wi, float& delta,
+                                                  float& offset, float& bits) {
   const float* t = A.stats + g * FQB200_STATS_STRIDE;
-  bits = A.has_widths ? static_cast<float>(A.widths[k]) : A.bit_alloc ? __ldg(t + 7) : static_cast<float>(A.num_bits);
+  bits = A.grid         ? static_cast<float>(A.widths[wi])
+         : A.has_widths ? static_cast<float>(A.widths[k])
+         : A.bit_alloc  ? __ldg(t + 7)
+                        : static_cast<float>(A.num_bits);
   solve_range(A.prior == 2 ? FQB200_RANGE_MINMAX : FQB200_RANGE_KSTD, A.positive != 0, A.num_bits, __ldg(A.mult + k),
               A.solve_f64 != 0, __ldg(t + 0), __ldg(t + 1), __ldg(t + 2), __ldg(t + 3), __ldg(t + (A.prior ? 4 : 3)), bits,
               delta, offset);
@@ -226,14 +236,16 @@ __global__ void __launch_bounds__(kCmThreads, 2) fq_clipmse_partial_kernel(const
   const CmSmem sm = cm_carve(cm_raw, A.K, A.Kpad, S);
   const int W = A.K + 1;
   for (unsigned long long u = blockIdx.x; u < A.units; u += gridDim.x) {
-    const unsigned long long sg = u / A.units_per_group, chunk = u % A.units_per_group;
+    const unsigned long long cu = u / static_cast<unsigned>(A.nw);   // unit = (group or slab, chunk, width index)
+    const unsigned long long sg = cu / A.units_per_group, chunk = cu % A.units_per_group;
+    const int wi = static_cast<int>(u - cu * static_cast<unsigned>(A.nw));
     bool fast = true;
     for (int i = threadIdx.x; i < A.Kpad * S; i += kCmThreads) {
       const int slot = i % S, k = i / S;
       unsigned long long g = LAY == 2 ? sg * kCmSlab + slot : sg;
       if (g >= A.groups) g = A.groups - 1;
       float d, o, b;
-      const LeafParam q = cm_candidate(A, g, k < A.K ? k : A.K - 1, d, o, b);
+      const LeafParam q = cm_candidate(A, g, k < A.K ? k : A.K - 1, wi, d, o, b);
       const Divisor dv = make_divisor(q.a);
       sm.scale[i] = q.a;
       sm.zp[i] = q.b;
@@ -245,10 +257,11 @@ __global__ void __launch_bounds__(kCmThreads, 2) fq_clipmse_partial_kernel(const
     if (__syncthreads_and(fast)) cm_unit<LAY, true>(A, sm, sg, chunk);
     else                         cm_unit<LAY, false>(A, sm, sg, chunk);
     __syncthreads();
+    const int wi2 = static_cast<int>(u % static_cast<unsigned>(A.nw)), row = A.nw * A.K + 1;
     for (int i = threadIdx.x; i < W * S; i += kCmThreads) {
       const int slot = i % S, k = i / S;
       const unsigned long long g = LAY == 2 ? sg * kCmSlab + slot : sg;
-      if (g < A.groups) A.partial[(g * A.units_per_group + chunk) * W + k] = sm.acc[i];
+      if (g < A.groups && (k > 0 || wi2 == 0)) A.partial[(g * A.units_per_group + chunk) * row + (k ? wi2 * A.K + k : 0)] = sm.acc[i];
     }
     __syncthreads();
   }
@@ -256,7 +269,7 @@ __global__ void __launch_bounds__(kCmThreads, 2) fq_clipmse_partial_kernel(const
 
 __global__ void __launch_bounds__(kCmThreads) fq_clipmse_finish_kernel(const __grid_constant__ ClipMseArgs A) {
   const unsigned long long g = blockIdx.x;
-  const int W = A.K + 1;
+  const int n = A.nw * A.K, W = n + 1;
   const double* p = A.partial + g * A.units_per_group * W;
   for (int k = threadIdx.x; k < W; k += kCmThreads) {
     double t = p[k];
@@ -264,10 +277,11 @@ __global__ void __launch_bounds__(kCmThreads) fq_clipmse_finish_kernel(const __g
     A.out[g * W + k] = t;
   }
   if (A.params) {
-    for (int k = threadIdx.x; k < A.K; k += kCmThreads) {
+    for (int j = threadIdx.x; j < n; j += kCmThreads) {
       float d, o, b;
-      const LeafParam q = cm_candidate(A, g, k, d, o, b);
-      float* dst = A.params + (g * A.K + k) * kCeParams;
+      const int wi = j / A.K;
+      const LeafParam q = cm_candidate(A, g, j - wi * A.K, wi, d, o, b);
+      float* dst = A.params + (g * n + j) * kCeParams;
       dst[0] = d; dst[1] = o; dst[2] = b; dst[3] = q.a; dst[4] = q.b; dst[5] = q.c;
     }
   }

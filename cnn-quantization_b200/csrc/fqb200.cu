@@ -1753,7 +1753,7 @@ size_t cliperr_workspace(int64_t outer, int64_t groups, int64_t inner, int chann
   return static_cast<size_t>(groups) * static_cast<size_t>(cliperr_units_per_group(outer, inner, channels_last)) * fqb::kCeSums * 8;
 }
 
-// clipping-MSE workspace: K + 1 float64 partials per (group, unit) (fq_clipmse.cuh)
+// clipping-MSE workspace: k + 1 float64 partials per (group, chunk), k = nw * K candidates (fq_clipmse.cuh)
 unsigned long long clipmse_units_per_group(int64_t outer, int64_t inner, int channels_last) {
   const unsigned long long n = static_cast<unsigned long long>(outer) * static_cast<unsigned long long>(inner);
   const unsigned long long per = channels_last ? fqb::kCmClRows : fqb::kCmChunk;
@@ -2656,6 +2656,57 @@ int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inne
                                 stream);
 }
 
+// the launch of fqb200_clip_mse_widths and fqb200_clip_mse_grid after their argument checks: K candidates per unit, nw
+// units per (group, chunk) - nw widths[i] of a grid launch, else 1 (widths, when given, one per candidate)
+static int clipmse_launch(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                          const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                          int32_t prior, const float* multipliers, int32_t K, const int32_t* widths, int32_t nw, bool grid,
+                          double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
+                          void* stream, const char* sizer) {
+  int rc = check_workspace(workspace, workspace_bytes, clipmse_workspace(outer, groups, inner, channels_last, nw * K), sizer);
+  if (rc != FQB200_OK) return rc;
+  DeviceInfo* di = nullptr;
+  rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  fqb::ClipMseArgs A;
+  memset(&A, 0, sizeof(A));
+  A.in = in;
+  A.stats = stats;
+  A.mult = multipliers;
+  A.outer = static_cast<unsigned long long>(outer);
+  A.groups = static_cast<unsigned long long>(groups);
+  A.inner = static_cast<unsigned long long>(inner);
+  A.channels_last = channels_last ? 1 : 0;
+  A.num_bits = num_bits;
+  A.positive = positive ? 1 : 0;
+  A.bit_alloc = bit_alloc ? 1 : 0;
+  A.solve_f64 = solve_f64 ? 1 : 0;
+  A.prior = prior;
+  A.K = K;
+  A.Kpad = (K + fqb::kCmTile - 1) / fqb::kCmTile * fqb::kCmTile;
+  A.has_widths = widths && !grid ? 1 : 0;
+  A.grid = grid ? 1 : 0;
+  A.nw = nw;
+  for (int k = 0; widths && k < (grid ? nw : K); ++k) A.widths[k] = static_cast<unsigned char>(widths[k]);
+  A.units_per_group = clipmse_units_per_group(outer, inner, channels_last);
+  A.units = A.units_per_group * (channels_last ? (A.groups + fqb::kCmSlab - 1) / fqb::kCmSlab : A.groups) *
+            static_cast<unsigned long long>(nw);
+  A.partial = static_cast<double*>(workspace);
+  A.out = out;
+  A.params = out_params;
+  const int grid_ctas = grid_for(A.units, di->sms * 2ull, max_ctas);
+  if (channels_last) {
+    fqb::fq_clipmse_partial_kernel<2><<<grid_ctas, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, fqb::kCmSlab), st>>>(A);
+  } else if (inner % 4 == 0 && aligned16(in)) {
+    fqb::fq_clipmse_partial_kernel<1><<<grid_ctas, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
+  } else {
+    fqb::fq_clipmse_partial_kernel<0><<<grid_ctas, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
+  }
+  fqb::fq_clipmse_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCmThreads, 0, st>>>(A);
+  return launched("clipping-MSE kernels");
+}
+
 int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                            const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
                            int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
@@ -2677,46 +2728,51 @@ int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64
     if (prior != 0 && prior != 1) return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b) or 1 (Gauss std)%s");
   }
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
-  int rc = check_workspace(workspace, workspace_bytes, clipmse_workspace(outer, groups, inner, channels_last, num_multipliers),
-                           "fqb200_clip_mse_workspace_bytes");
-  if (rc != FQB200_OK) return rc;
-  DeviceInfo* di = nullptr;
-  rc = get_device(&di);
-  if (rc != FQB200_OK) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  fqb::ClipMseArgs A;
-  memset(&A, 0, sizeof(A));
-  A.in = in;
-  A.stats = stats;
-  A.mult = multipliers;
-  A.outer = static_cast<unsigned long long>(outer);
-  A.groups = static_cast<unsigned long long>(groups);
-  A.inner = static_cast<unsigned long long>(inner);
-  A.channels_last = channels_last ? 1 : 0;
-  A.num_bits = num_bits;
-  A.positive = positive ? 1 : 0;
-  A.bit_alloc = bit_alloc ? 1 : 0;
-  A.solve_f64 = solve_f64 ? 1 : 0;
-  A.prior = prior;
-  A.K = num_multipliers;
-  A.Kpad = (num_multipliers + fqb::kCmTile - 1) / fqb::kCmTile * fqb::kCmTile;
-  A.has_widths = widths ? 1 : 0;
-  for (int k = 0; widths && k < num_multipliers; ++k) A.widths[k] = static_cast<unsigned char>(widths[k]);
-  A.units_per_group = clipmse_units_per_group(outer, inner, channels_last);
-  A.units = A.units_per_group * (channels_last ? (A.groups + fqb::kCmSlab - 1) / fqb::kCmSlab : A.groups);
-  A.partial = static_cast<double*>(workspace);
-  A.out = out;
-  A.params = out_params;
-  const int grid = grid_for(A.units, di->sms * 2ull, max_ctas);
-  if (channels_last) {
-    fqb::fq_clipmse_partial_kernel<2><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, fqb::kCmSlab), st>>>(A);
-  } else if (inner % 4 == 0 && aligned16(in)) {
-    fqb::fq_clipmse_partial_kernel<1><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
-  } else {
-    fqb::fq_clipmse_partial_kernel<0><<<grid, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, 1), st>>>(A);
+  return clipmse_launch(in, outer, groups, inner, channels_last, stats, num_bits, positive, bit_alloc, solve_f64, prior,
+                        multipliers, num_multipliers, widths, 1, false, out, out_params, workspace, workspace_bytes, max_ctas,
+                        stream, "fqb200_clip_mse_workspace_bytes");
+}
+
+// the layouts, multiplier and width counts fqb200_clip_mse_grid takes (argument errors as a message, nullptr when fine)
+static const char* clipmse_grid_bad_args(int64_t outer, int64_t groups, int64_t inner, int channels_last, int32_t m,
+                                         int32_t w) {
+  const char* bad = clipmse_bad_args(outer, groups, inner, channels_last, m);
+  if (bad) return bad;
+  if (w < 1 || w > 9) return "num_widths must be in 1..9%s";
+  return nullptr;
+}
+
+size_t fqb200_clip_mse_grid_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                                            int32_t num_multipliers, int32_t num_widths) {
+  g_err[0] = 0;
+  const char* bad = clipmse_grid_bad_args(outer, groups, inner, channels_last, num_multipliers, num_widths);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  return clipmse_workspace(outer, groups, inner, channels_last, num_widths * num_multipliers);
+}
+
+int fqb200_clip_mse_grid(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                         const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                         int32_t prior, const float* multipliers, int32_t num_multipliers, const int32_t* widths,
+                         int32_t num_widths, double* out, float* out_params, void* workspace, size_t workspace_bytes,
+                         int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  const char* bad = clipmse_grid_bad_args(outer, groups, inner, channels_last, num_multipliers, num_widths);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!in || !stats || !multipliers || !widths || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (num_bits < 1 || num_bits > 8) return fail(FQB200_ERR_INVALID, "num_bits must be in 1..8%s");
+  if (bit_alloc) return fail(FQB200_ERR_INVALID, "widths and bit_alloc are two sources of widths: pass one%s");
+  if (prior != 0 && prior != 1)
+    return fail(FQB200_ERR_INVALID, "prior must be 0 (Laplace b) or 1 (Gauss std): min/max ignores the multipliers%s");
+  unsigned seen = 0;
+  for (int i = 0; i < num_widths; ++i) {
+    if (widths[i] < 0 || widths[i] > 8) return fail(FQB200_ERR_INVALID, "widths must be in 0..8%s");
+    if (seen & (1u << widths[i])) return fail(FQB200_ERR_INVALID, "widths must be distinct%s");
+    seen |= 1u << widths[i];
   }
-  fqb::fq_clipmse_finish_kernel<<<static_cast<unsigned>(groups), fqb::kCmThreads, 0, st>>>(A);
-  return launched("clipping-MSE kernels");
+  if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
+  return clipmse_launch(in, outer, groups, inner, channels_last, stats, num_bits, positive, 0, solve_f64, prior,
+                        multipliers, num_multipliers, widths, num_widths, true, out, out_params, workspace, workspace_bytes,
+                        max_ctas, stream, "fqb200_clip_mse_grid_workspace_bytes");
 }
 
 // the requests fqb200_kmeans1d takes (argument errors as a message, nullptr when they are fine)

@@ -406,6 +406,9 @@ class IntQuantizer(object):
         """`-bap mse`: float32 [C] widths minimising the sum of the layer's measured per-channel errors (bit_mse.pkl,
         collected with collect_bits under this run's clipping rule) for the budget of ``target`` bits per channel."""
         from .bit_alloc import allocate
+        if self.clipping == "mse":
+            raise NotImplementedError("-bap mse under -c mse picks each channel's width together with its clipping value "
+                                      "(_joint_alpha_from_stats), not the width alone")
         if self.kld or self.clipping not in ("laplace", "gaus", "no"):
             raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus or no, not %s"
                                       % ("-kld" if self.kld else "-c " + self.clipping))
@@ -507,7 +510,10 @@ class IntQuantizer(object):
     def _mse_alpha_from_stats(self, stat_id, per_channel, dev):
         """`-c mse`: per group, alpha = m* times the summary b (or std, for curves collected with mse_prior="gaus"), m* the
         multiplier at the minimum of the group's collected clipping-MSE curve (ties: the smaller multiplier) - in fp32 per
-        channel, in float64 per tensor, like the Laplace alpha.  Bits as in `-c laplace`."""
+        channel, in float64 per tensor, like the Laplace alpha.  Bits as in `-c laplace`; with `-baa -bap mse` the width
+        and the clipping value of each channel come together from the joint tables (``_joint_alpha_from_stats``)."""
+        if per_channel and self.bit_alloc_act and self.num_bits <= 4 and self.bit_alloc_prior == "mse":
+            return self._joint_alpha_from_stats(stat_id, dev)
         if self.mse_curves is None:
             raise KeyError("-c mse needs the clipping-MSE curve of layer %r: collect it with collect_mse=True" % (stat_id,))
         m, prior = self.mse_curves.best(stat_id)
@@ -525,6 +531,28 @@ class IntQuantizer(object):
             raise ValueError("-c mse: the curve of %r is per channel (%d groups) but the layer is quantized per tensor"
                              % (stat_id, m.size))
         return float(scale) * float(m[0]), bits
+
+    def _joint_alpha_from_stats(self, stat_id, dev):
+        """`-c mse -baa -bap mse`: (float32 [C] alpha, float32 [C] widths) of a per-channel, bit-allocated call site.  The
+        widths are bit_alloc.allocate's on the layer's joint tables (bit_mse.pkl collected with collect_bits under -c
+        mse: per channel and width, the error at the best multiplier), and alpha_c = m_w[c, w_c] * scale_c in fp32, scale
+        the summary b (or std, for tables collected with mse_prior="gaus"), as `-c mse` forms it."""
+        from .bit_alloc import allocate
+        if self.bit_tables is None:
+            raise KeyError("-bap mse needs the per-channel error tables of layer %r: collect them with collect_bits=True"
+                           % (stat_id,))
+        mse, rule = self.bit_tables.table(stat_id)
+        if rule != "mse":
+            raise ValueError("-c mse -bap mse: the tables of %r were measured under -c %s; collect them under -c mse with "
+                             "collect_bits=True" % (stat_id, rule))
+        m, prior = self.bit_tables.multipliers_of(stat_id)
+        scale = np.asarray(self._stat(stat_id, "b" if prior == "laplace" else "std", "mean"), dtype=np.float32).reshape(-1)
+        if mse.shape[0] != scale.size:
+            raise ValueError("-bap mse: the table of %r has %d groups, the statistics %d channels"
+                             % (stat_id, mse.shape[0], scale.size))
+        widths = allocate(mse, self.bit_alloc_target_act)
+        alpha = scale * m[np.arange(scale.size), widths]
+        return alpha, torch.tensor(widths, dtype=torch.float32, device=dev)
 
     # ------------------------------------------------------------------------------------------
     # dispatch targets

@@ -14,6 +14,7 @@ call sites, same ``quantize_instant`` / ``quantize_model`` semantics, but
 SURVEY.md 8f rank 1) and ``-bca`` (rank 2, use mode only) are implemented on top of the same kernels.
 """
 import argparse
+import os
 from itertools import count
 
 import torch
@@ -38,7 +39,10 @@ def make_args(**over):
     `-c mse` in use mode clips at the minimum of those curves), ``collect_bits`` (also write, for every call site `-sm use`
     quantizes per channel with bit allocation, the error of its quantizer on each channel at every width 0..8; needs
     ``per_channel_quant_act``, ``bit_alloc_act`` and clipping laplace, gaus or no; ``bit_alloc_prior="mse"`` (`-bap mse`) then allocates the
-    widths that minimise the sum of those errors, and allocates weight widths from the weights' own errors) and
+    widths that minimise the sum of those errors, and allocates weight widths from the weights' own errors.  With
+    clipping "mse" and ``collect_mse`` - the curves clip the call sites without allocation - it measures every width at
+    every ``mse_multipliers`` value instead, and `-c mse -bap mse` picks each channel's width and clipping value
+    together) and
     ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms; "angle", the
     pairwise sample angles of its angle_stats module, which the reference selects by editing an import; or "noise", the
     per-sample quantization error statistics of its measure_statistics module, which the reference cannot run)."""
@@ -424,14 +428,16 @@ class QuantizationManagerInference(object):
                                               ("a qtype", args.qtype is not None),
                                               ("per_channel_quant_act", args.per_channel_quant_act),
                                               ("bit_alloc_act", args.bit_alloc_act),
-                                              ("clipping laplace, gaus or no", args.clipping in ("laplace", "gaus", "no")))
+                                              ("clipping laplace, gaus or no (or mse with collect_mse)",
+                                               args.clipping in ("laplace", "gaus", "no")
+                                               or (args.clipping == "mse" and self.collect_mse)))
                        if not ok]
             if missing:
                 raise ValueError("collect_bits measures the per-channel error tables of -sm collect: it needs %s"
                                  % ", ".join(missing))
         bap_mse = getattr(args, "bit_alloc_prior", None) == "mse"
-        if bap_mse and (args.kld_threshold or args.clipping in ("mix", "mse")):
-            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus or no, not %s"
+        if bap_mse and (args.kld_threshold or args.clipping == "mix"):
+            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus, no or mse, not %s"
                                       % ("-kld" if args.kld_threshold else "-c " + args.clipping))
         if bap_mse and getattr(args, "mid_thread_quant", False):
             raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
@@ -465,17 +471,25 @@ class QuantizationManagerInference(object):
                                                       getattr(args, "mse_prior", "laplace"), base_dir=base)
                 if self.collect_bits:
                     from .statistics import BitMseStatistics
-                    self.bit_mse = BitMseStatistics(sf, args.clipping, base_dir=base)
+                    self.bit_mse = BitMseStatistics(sf, args.clipping, base_dir=base,
+                                                    multipliers=getattr(args, "mse_multipliers", None),
+                                                    prior=getattr(args, "mse_prior", "laplace"))
             else:
+                if bap_mse:   # read on first use: a missing layer raises KeyError naming collect_bits there
+                    from .statistics import BitMseStatistics
+                    self.bit_mse = BitMseStatistics(sf, base_dir=base, load=True)
+                    if args.clipping == "mse" and args.bit_alloc_act and not os.path.exists(self.bit_mse.path):
+                        # without joint tables the only combination left is -c mse's curves at separately measured
+                        # widths, which is not implemented: -c mse -bap mse picks width and clipping value together
+                        raise NotImplementedError("-c mse -baa -bap mse picks each channel's width and clipping value "
+                                                  "from joint tables, and there are none at %s: collect them under -c mse "
+                                                  "with collect_bits=True and collect_mse=True" % self.bit_mse.path)
                 if args.per_channel_quant_act:
                     self._sm_channel = StatisticManagerPerChannel(sf, load_stats=True, base_dir=base)
                 self._sm_tensor = StatisticManager(sf, load_stats=True, base_dir=base)
                 if args.clipping == "mse":   # read on first use: a missing file raises KeyError naming collect_mse there
                     from .statistics import ClipMseStatistics
                     self.clip_mse = ClipMseStatistics(sf, base_dir=base, load=True)
-                if bap_mse:   # read on first use: a missing file raises KeyError naming collect_bits there
-                    from .statistics import BitMseStatistics
-                    self.bit_mse = BitMseStatistics(sf, base_dir=base, load=True)
         self.fused_relu = args.arch is not None and (args.arch in FUSED_RELU_ARCHS or "squeezenet" in args.arch)
         self.ignore_ids = []
         self.quantizers = {}

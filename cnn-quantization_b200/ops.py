@@ -636,25 +636,11 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
     (0 as the lower bound when ``positive``), which ignores the multipliers.  Deterministic, no host synchronisation; with
     ``want_params`` also returns the [groups, K, 6] candidate parameters (delta, offset, bits, scale, zero point, qmax).
     Recorded in the launch profile under mode 'R' (one read of the tensor)."""
-    _require_cuda_f32(x, "tensor")
-    outer, groups, inner = (int(v) for v in layout)
-    if outer * groups * inner != x.numel():
-        raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
-    if prior not in CLIP_MSE_PRIORS or (prior == "minmax" and widths is None):
-        raise ValueError("prior must be one of %s (minmax with widths only), got %r" % (sorted(CLIP_MSE_PRIORS), prior))
-    if channels_last:
-        if not cl_eligible(x, layout):
-            raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
-    elif not (outer == 1 and groups == 1 and dense(x)):
-        x = x.contiguous()   # one group: any dense memory order; per channel: NCHW order
-    if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
-            or tuple(table.shape) != (groups, L.STATS_STRIDE)):
-        raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
-    table = table.contiguous()
-    mult = torch.as_tensor(multipliers, dtype=torch.float32).reshape(-1).to(x.device).contiguous()
+    bad_prior = prior not in CLIP_MSE_PRIORS or (prior == "minmax" and widths is None)
+    x, table, mult, (outer, groups, inner) = _clip_mse_inputs(
+        "clip_mse", x, table, layout, channels_last, multipliers,
+        bad_prior and "prior must be one of %s (minmax with widths only), got %r" % (sorted(CLIP_MSE_PRIORS), prior))
     k = mult.numel()
-    if not 1 <= k <= 256:
-        raise ValueError("clip_mse takes 1..256 multipliers, got %d" % k)
     if widths is not None:
         widths = np.ascontiguousarray(widths, dtype=np.int32).reshape(-1)   # host values, validated by the library
         if widths.size != k:
@@ -677,6 +663,63 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
         _launch(dev, timed, lib.fqb200_clip_mse, *head, *tail)
     else:
         _launch(dev, timed, lib.fqb200_clip_mse_widths, *head, widths.ctypes.data, *tail)
+    return (out, params) if want_params else out
+
+
+def _clip_mse_inputs(name, x, table, layout, channels_last, multipliers, bad_prior):
+    """(x in the memory order the launch reads, contiguous table, float32 device multipliers, layout) of clip_mse and
+    clip_mse_grid, after their common checks; ``bad_prior``, when not false, is the ValueError of an unusable prior."""
+    _require_cuda_f32(x, "tensor")
+    outer, groups, inner = (int(v) for v in layout)
+    if outer * groups * inner != x.numel():
+        raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
+    if bad_prior:
+        raise ValueError(bad_prior)
+    if channels_last:
+        if not cl_eligible(x, layout):
+            raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
+    elif not (outer == 1 and groups == 1 and dense(x)):
+        x = x.contiguous()   # one group: any dense memory order; per channel: NCHW order
+    if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
+            or tuple(table.shape) != (groups, L.STATS_STRIDE)):
+        raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
+    mult = torch.as_tensor(multipliers, dtype=torch.float32).reshape(-1).to(x.device).contiguous()
+    if not 1 <= mult.numel() <= 256:
+        raise ValueError("%s takes 1..256 multipliers, got %d" % (name, mult.numel()))
+    return x, table.contiguous(), mult, (outer, groups, inner)
+
+
+def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multipliers, widths, prior="laplace", solve_f64=None,
+                  want_params=False, max_ctas=0):
+    """C ABI fqb200_clip_mse_grid: ``clip_mse`` over every pair of W = len(``widths``) (1..9 distinct values in 0..8) bit
+    widths and M = len(``multipliers``) (1..256) clipping values, the joint width-and-clip tables of `-c mse -bap mse`, as
+    a [groups, 1 + W * M] float64 device tensor: column 0 sum x^2, column 1 + i * M + k the sum of candidate (widths[i],
+    multipliers[k]) - bit for bit ``clip_mse(..., [multipliers[k]], widths=[widths[i]])``.  ``prior`` "laplace" or "gaus"
+    (min/max ignores the multipliers); the other arguments as in ``clip_mse``.  With ``want_params`` also returns the
+    [groups, W * M, 6] candidate parameters.  Recorded in the launch profile under mode 'R'."""
+    x, table, mult, (outer, groups, inner) = _clip_mse_inputs(
+        "clip_mse_grid", x, table, layout, channels_last, multipliers,
+        prior not in ("laplace", "gaus") and "clip_mse_grid: prior must be 'laplace' or 'gaus', got %r" % (prior,))
+    m = mult.numel()
+    widths = np.ascontiguousarray(widths, dtype=np.int32).reshape(-1)   # host values, validated by the library
+    if not 1 <= widths.size <= 9:
+        raise ValueError("clip_mse_grid takes 1..9 widths, got %d" % widths.size)
+    n = widths.size * m
+    lib = L.load()
+    dev = x.device
+    if solve_f64 is None:
+        solve_f64 = groups == 1
+    out = torch.empty((groups, n + 1), dtype=torch.float64, device=dev)
+    params = torch.empty((groups, n, 6), dtype=torch.float32, device=dev) if want_params else None
+    if x.numel() == 0:
+        out.zero_()
+        return (out, params) if want_params else out
+    ws = _own_workspace(dev, lib.fqb200_clip_mse_grid_workspace_bytes(outer, groups, inner, int(bool(channels_last)), m,
+                                                                      widths.size))
+    _launch(dev, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse_grid, x.data_ptr(),
+            outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), 0,
+            int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), m, widths.ctypes.data, widths.size,
+            out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
     return (out, params) if want_params else out
 
 

@@ -570,14 +570,18 @@ def _clip_table(t, cfg, channels_last):
                              bit_alloc_target=cfg.bit_alloc_target, stats_only=True, channels_last=channels_last)
 
 
-def best_multipliers(multipliers, mse):
-    """Per row of ``mse`` ([G, K], one column per multiplier) the multiplier of the smallest MSE; ties go to the smaller
+def best_columns(multipliers, mse):
+    """Per row of ``mse`` ([G, K], one column per multiplier) the column of the smallest MSE; ties go to the smaller
     multiplier and NaN never wins (a row of NaN gives the smallest multiplier)."""
-    m = np.asarray(multipliers, dtype=np.float32)
-    order = np.argsort(m, kind="stable")
+    order = np.argsort(np.asarray(multipliers, dtype=np.float32), kind="stable")
     e = np.asarray(mse, dtype=np.float64)[:, order]
     e = np.where(np.isnan(e), np.inf, e)
-    return m[order][np.argmin(e, axis=1)]
+    return order[np.argmin(e, axis=1)]
+
+
+def best_multipliers(multipliers, mse):
+    """Per row of ``mse`` ([G, K], one column per multiplier) the multiplier of the smallest MSE (``best_columns``)."""
+    return np.asarray(multipliers, dtype=np.float32)[best_columns(multipliers, mse)]
 
 
 class ClipMseStatistics(object):
@@ -700,7 +704,7 @@ class ClipMseStatistics(object):
         return best_multipliers(m, df[["mse_%d" % j for j in range(len(m))]].to_numpy()), self.curves["prior"]
 
 
-BIT_RULES = ("laplace", "gaus", "no")
+BIT_RULES = ("laplace", "gaus", "no", "mse")
 
 
 def bit_candidates(rule, positive, num_bits):
@@ -716,24 +720,34 @@ def bit_candidates(rule, positive, num_bits):
         return [(ALPHA_GAUS_POSITIVE if positive else ALPHA_GAUS)[num_bits]] * 9, "gaus"
     if rule == "no":
         return [0.0] * 9, "minmax"
-    raise ValueError("bit allocation tables are measured under clipping %s, got %r" % (list(BIT_RULES), rule))
+    raise ValueError("bit allocation tables are measured under clipping %s, got %r" % (list(BIT_RULES[:3]), rule))
 
 
 class BitMseStatistics(object):
     """Per-channel error tables of bit allocation (`collect_bits`): ``save_table(t, tag, id, cfg)`` adds, for a call site
     whose quantizer ``cfg`` (a ClipErrConfig) quantizes per channel with bit allocation, the float64 sums of one
     ops.clip_mse launch over the 9 candidates of ``bit_candidates(rule, ...)`` and the channels' b and std to device
-    accumulators; other call sites are skipped.  ``__exit__`` writes bit_mse.pkl and alloc.csv.  With ``load`` the instance
-    reads bit_mse.pkl instead (on first use), for `-bap mse`."""
+    accumulators; other call sites are skipped.  Under rule "mse" (`-c mse`, the joint width-and-clip search) the launch is
+    one ops.clip_mse_grid over widths 0..8 times ``multipliers`` (alpha = m * b with ``prior`` "laplace", m * std with
+    "gaus"), and each width's error is the one at its best multiplier (``best_columns``).  ``__exit__`` writes bit_mse.pkl
+    and alloc.csv.  With ``load`` the instance reads bit_mse.pkl instead (on first use), for `-bap mse`."""
 
-    def __init__(self, folder, rule=None, base_dir=None, load=False):
+    def __init__(self, folder, rule=None, base_dir=None, load=False, multipliers=None, prior="laplace"):
         if not load and rule not in BIT_RULES:
             raise ValueError("collect_bits measures under clipping %s, got %r" % (list(BIT_RULES), rule))
         self.folder = os.path.join(base_dir or default_base_dir(), "bit_mse", folder)
         self.rule = rule
+        if rule == "mse":
+            if prior not in ("gaus", "laplace"):
+                raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
+            self.multipliers = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers,
+                                          dtype=np.float32).reshape(-1)
+            if not 1 <= self.multipliers.size <= 256:
+                raise ValueError("mse_multipliers: 1..256 values, got %d" % self.multipliers.size)
+            self.prior = prior
         self.load = load
         self.tables = None
-        self.acc = {}    # id -> (sums [G, 10], b / std sums [G, 2], float64 device tensors, batches)
+        self.acc = {}    # id -> (sums [G, 10] or, rule "mse", [G, 1 + 9 M], b / std sums [G, 2], float64 device tensors, batches)
         self.meta = {}   # id -> (internal_name, ClipErrConfig, elements per channel and batch)
         self._mult_dev = {}
 
@@ -748,13 +762,20 @@ class BitMseStatistics(object):
         if not cl:
             t = t.contiguous()
         table = ops.fused(t, layout, num_bits=8, stats_only=True, channels_last=cl)
-        mults, prior = bit_candidates(self.rule, cfg.positive, cfg.num_bits)
-        key = (t.device, bool(cfg.positive), cfg.num_bits)
-        mult = self._mult_dev.get(key)
-        if mult is None:
-            mult = self._mult_dev[key] = torch.tensor(mults, dtype=torch.float32, device=t.device)
-        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=prior, widths=range(9),
-                            solve_f64=False)
+        if self.rule == "mse":
+            mult = self._mult_dev.get(t.device)
+            if mult is None:
+                mult = self._mult_dev[t.device] = torch.from_numpy(self.multipliers).to(t.device)
+            sums = ops.clip_mse_grid(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, range(9), prior=self.prior,
+                                     solve_f64=False)
+        else:
+            mults, prior = bit_candidates(self.rule, cfg.positive, cfg.num_bits)
+            key = (t.device, bool(cfg.positive), cfg.num_bits)
+            mult = self._mult_dev.get(key)
+            if mult is None:
+                mult = self._mult_dev[key] = torch.tensor(mults, dtype=torch.float32, device=t.device)
+            sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=prior, widths=range(9),
+                                solve_f64=False)
         scales = table[:, 3:5].double()
         prev = self.acc.get(id)
         if prev is None:
@@ -777,50 +798,71 @@ class BitMseStatistics(object):
         from .int_quantizer import IntQuantizer
         flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
         out = {"rule": self.rule}
+        joint = self.rule == "mse"
+        if joint:
+            out.update(multipliers=self.multipliers.astype(np.float64), prior=self.prior)
         rows = []
         pos = 0
         for id in list(self.acc):
             sums, _, batches = self.acc[id]
-            g = sums.shape[0]
-            s = flat[pos:pos + g * 10].reshape(g, 10)
-            pos += g * 10
+            g, n = sums.shape
+            s = flat[pos:pos + g * n].reshape(g, n)
+            pos += g * n
             sc = flat[pos:pos + g * 2].reshape(g, 2) / batches
             pos += g * 2
             tag, cfg, per_batch = self.meta[id]
             count = np.full(g, float(per_batch * batches))
-            mse = s[:, 1:] / count[:, None]
             df = pd.DataFrame({"count": count, "b": sc[:, 0], "std": sc[:, 1], "positive": np.full(g, bool(cfg.positive))})
-            out[id] = pd.concat([df, pd.DataFrame(mse, columns=["mse_w%d" % w for w in range(9)])], axis=1)
+            if joint:   # each width's sum at its best multiplier
+                grid = s[:, 1:].reshape(g, 9, -1)
+                best = np.stack([best_columns(self.multipliers, grid[:, w]) for w in range(9)], 1)
+                sse = np.take_along_axis(grid, best[:, :, None], 2)[:, :, 0]
+            else:
+                sse = s[:, 1:]
+            mse = sse / count[:, None]
+            cols = [df, pd.DataFrame(mse, columns=["mse_w%d" % w for w in range(9)])]
+            if joint:
+                cols.append(pd.DataFrame(self.multipliers[best], columns=["m_w%d" % w for w in range(9)]))
+            out[id] = pd.concat(cols, axis=1)
             prior = sc[:, 0] if cfg.bit_alloc_prior == L.PRIOR_B else sc[:, 1]
             analytic = IntQuantizer.get_bits_alloc_fixed_target(torch.from_numpy(prior.astype(np.float32)),
                                                                 cfg.bit_alloc_target, cfg.bit_alloc_round)
             allocations = (np.full(g, cfg.num_bits), analytic.numpy().astype(np.int64), allocate(mse, cfg.bit_alloc_target))
             row = [id, tag, g, cfg.bit_alloc_target]
             for w in allocations:
-                row += [int(w.sum()), float(s[np.arange(g), 1 + w].sum() / count.sum())]
+                row += [int(w.sum()), float(sse[np.arange(g), w].sum() / count.sum())]
             rows.append(row)
         if os.path.exists(self.folder):
             shutil.rmtree(self.folder)
         os.makedirs(self.folder)
-        with open(os.path.join(self.folder, "bit_mse.pkl"), "wb") as f:
+        with open(self.path, "wb") as f:
             pickle.dump(out, f)
         pd.DataFrame(rows, columns=ALLOC_COLUMNS).to_csv(os.path.join(self.folder, "alloc.csv"), index=False)
         self.acc, self.meta = {}, {}
 
     # -- use (`-bap mse`) --------------------------------------------------------------------------------------------
+    @property
+    def path(self):
+        return os.path.join(self.folder, "bit_mse.pkl")
+
     def table(self, id):
         """(float64 [C, 9] per-element MSE of widths 0..8, rule) collected for ``id``; KeyError naming collect_bits when
         there is none."""
         if self.tables is None:
-            path = os.path.join(self.folder, "bit_mse.pkl")
-            if not os.path.exists(path):
-                raise KeyError("-bap mse needs the per-channel error tables at %s: collect them with collect_bits=True" % path)
-            with open(path, "rb") as f:
+            if not os.path.exists(self.path):
+                raise KeyError("-bap mse needs the per-channel error tables at %s: collect them with collect_bits=True"
+                               % self.path)
+            with open(self.path, "rb") as f:
                 self.tables = pickle.load(f)
         df = self.tables.get(id)
         if df is None:
             raise KeyError("-bap mse needs the per-channel error table of layer %r: collect it with collect_bits=True" % (id,))
         return df[["mse_w%d" % w for w in range(9)]].to_numpy(dtype=np.float64), self.tables["rule"]
+
+    def multipliers_of(self, id):
+        """(float32 [C, 9] best multiplier of each width, prior) of a joint table (rule "mse") collected for ``id``."""
+        self.table(id)
+        return self.tables[id][["m_w%d" % w for w in range(9)]].to_numpy(dtype=np.float32), self.tables["prior"]
 
 
 ALLOC_COLUMNS = ["id", "internal_name", "groups", "target", "bits_uniform", "mse_uniform", "bits_analytic", "mse_analytic",

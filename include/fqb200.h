@@ -407,6 +407,29 @@ int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64
  * take). */
 size_t fqb200_clip_mse_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                                        int32_t num_multipliers);
+/*
+ * The joint width-and-clip tables of `-c mse -bap mse`: fqb200_clip_mse over every pair of W = num_widths (1..9) distinct
+ * widths (0..8) and M = num_multipliers (1..256) multipliers in one launch.  Candidate j = i * M + k quantizes at
+ * widths[i] and clips at alpha = multipliers[k] * b (prior 0) or * std (prior 1):
+ *   out[g * (1 + W * M) + 0] = sum x^2;  out[g * (1 + W * M) + 1 + j] = sum (x - q_j)^2
+ * and every column has the bits of fqb200_clip_mse_widths on the same (width, multiplier) pair, on every run and for
+ * every max_ctas.  `widths` is a host array (read before the call returns), `multipliers` a device array; the other
+ * arguments as in fqb200_clip_mse_widths.  out_params (optional): [groups][W * M][6].  Each work unit runs one width's M
+ * candidates, so a unit's shared memory is that of an M-candidate launch; x is read from HBM once per chunk and from L2
+ * by the chunk's other W - 1 units.  Workspace (fqb200_clip_mse_grid_workspace_bytes): groups x chunks x (1 + W * M) x 8
+ * bytes, computed from the shapes - e.g. 64 x 784 x 1126 x 8 = 452 MB for a channels-last 512 x 64 x 112 x 112 tensor at
+ * 9 x 125 candidates.  FQB200_ERR_INVALID, before any CUDA call: the layout errors of fqb200_clip_error, M outside
+ * 1..256, W outside 1..9, a width outside 0..8 or repeated, prior other than 0 or 1 (min/max ignores the multipliers: it
+ * has no grid), bit_alloc set, a null x, stats, multipliers, widths or out, bad num_bits, max_ctas < 0.
+ */
+int fqb200_clip_mse_grid(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                         const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                         int32_t prior, const float* multipliers, int32_t num_multipliers, const int32_t* widths,
+                         int32_t num_widths, double* out, float* out_params, void* workspace, size_t workspace_bytes,
+                         int32_t max_ctas, void* stream);
+/* Workspace of fqb200_clip_mse_grid in bytes (0 and fqb200_last_error() on a layout, M or W it does not take). */
+size_t fqb200_clip_mse_grid_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                                            int32_t num_multipliers, int32_t num_widths);
 
 /*
  * 1-D k-means quantization of one weight tensor (pytorch_quantizer/quantization/kmeans_quantization.py:14-30): scikit-learn
