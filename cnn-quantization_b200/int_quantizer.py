@@ -406,24 +406,36 @@ class IntQuantizer(object):
         """`-bap mse`: float32 [C] widths minimising the sum of the layer's measured per-channel errors (bit_mse.pkl,
         collected with collect_bits under this run's clipping rule) for the budget of ``target`` bits per channel."""
         from .bit_alloc import allocate
+        from .statistics import BIT_RULES
         if self.clipping == "mse":
             raise NotImplementedError("-bap mse under -c mse picks each channel's width together with its clipping value "
                                       "(_joint_alpha_from_stats), not the width alone")
-        if self.kld or self.clipping not in ("laplace", "gaus", "no"):
-            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus or no, not %s"
-                                      % ("-kld" if self.kld else "-c " + self.clipping))
+        if self.kld or self.clipping not in BIT_RULES:
+            raise NotImplementedError("-bap mse allocates from tables measured under -c %s, not %s"
+                                      % (", ".join(BIT_RULES[:3]), "-kld" if self.kld else "-c " + self.clipping))
+        mse = self._bit_table(stat_id, self.clipping)[0]
+        return torch.tensor(allocate(mse, target), dtype=torch.float32, device=device)
+
+    def _bit_table(self, stat_id, rule):
+        """(float64 [C, 9] errors of widths 0..8, float32 [C] scale, float32 [C, 9] best multipliers of a joint table
+        (``rule`` "mse") or None) of the layer's `-bap mse` table, checked to exist, to be measured under ``rule`` and to
+        have a row per channel of the summary scale: b (std for mse_prior "gaus") for a joint table, else max."""
         if self.bit_tables is None:
             raise KeyError("-bap mse needs the per-channel error tables of layer %r: collect them with collect_bits=True"
                            % (stat_id,))
-        mse, rule = self.bit_tables.table(stat_id)
-        if rule != self.clipping:
-            raise ValueError("-bap mse: the tables of %r were measured under -c %s, this run clips with -c %s"
-                             % (stat_id, rule, self.clipping))
-        channels = np.size(self._stat(stat_id, "max", "mean"))
-        if mse.shape[0] != channels:
+        mse, measured = self.bit_tables.table(stat_id)
+        if measured != rule:
+            raise ValueError("-bap mse: the tables of %r were measured under -c %s, this run clips with -c %s; collect "
+                             "them under -c %s with collect_bits=True" % (stat_id, measured, rule, rule))
+        m, stat = None, "max"
+        if rule == "mse":
+            m, prior = self.bit_tables.multipliers_of(stat_id)
+            stat = "b" if prior == "laplace" else "std"
+        scale = np.asarray(self._stat(stat_id, stat, "mean"), dtype=np.float32).reshape(-1)
+        if mse.shape[0] != scale.size:
             raise ValueError("-bap mse: the table of %r has %d groups, the statistics %d channels"
-                             % (stat_id, mse.shape[0], channels))
-        return torch.tensor(allocate(mse, target), dtype=torch.float32, device=device)
+                             % (stat_id, mse.shape[0], scale.size))
+        return mse, scale, m
 
     def _clipping_params_from_stats(self, tensor, stat_id, clip_type):
         """(delta, offset, bits, per_channel) of gemmlowpClippingQuantize in use mode (int_quantizer.py:327-359 with
@@ -538,18 +550,7 @@ class IntQuantizer(object):
         mse: per channel and width, the error at the best multiplier), and alpha_c = m_w[c, w_c] * scale_c in fp32, scale
         the summary b (or std, for tables collected with mse_prior="gaus"), as `-c mse` forms it."""
         from .bit_alloc import allocate
-        if self.bit_tables is None:
-            raise KeyError("-bap mse needs the per-channel error tables of layer %r: collect them with collect_bits=True"
-                           % (stat_id,))
-        mse, rule = self.bit_tables.table(stat_id)
-        if rule != "mse":
-            raise ValueError("-c mse -bap mse: the tables of %r were measured under -c %s; collect them under -c mse with "
-                             "collect_bits=True" % (stat_id, rule))
-        m, prior = self.bit_tables.multipliers_of(stat_id)
-        scale = np.asarray(self._stat(stat_id, "b" if prior == "laplace" else "std", "mean"), dtype=np.float32).reshape(-1)
-        if mse.shape[0] != scale.size:
-            raise ValueError("-bap mse: the table of %r has %d groups, the statistics %d channels"
-                             % (stat_id, mse.shape[0], scale.size))
+        mse, scale, m = self._bit_table(stat_id, "mse")
         widths = allocate(mse, self.bit_alloc_target_act)
         alpha = scale * m[np.arange(scale.size), widths]
         return alpha, torch.tensor(widths, dtype=torch.float32, device=dev)

@@ -423,22 +423,22 @@ class QuantizationManagerInference(object):
         self.clip_mse = None
         # `collect_bits`: the collect hooks also measure the per-channel error tables `-bap mse` allocates from
         self.collect_bits = bool(getattr(args, "collect_bits", False))
+        from .statistics import BIT_RULES
         if self.collect_bits:
             missing = [what for what, ok in (("stats_mode='collect'", self.stats_mode == "collect"),
                                               ("a qtype", args.qtype is not None),
                                               ("per_channel_quant_act", args.per_channel_quant_act),
                                               ("bit_alloc_act", args.bit_alloc_act),
                                               ("clipping laplace, gaus or no (or mse with collect_mse)",
-                                               args.clipping in ("laplace", "gaus", "no")
-                                               or (args.clipping == "mse" and self.collect_mse)))
+                                               args.clipping in BIT_RULES and (args.clipping != "mse" or self.collect_mse)))
                        if not ok]
             if missing:
                 raise ValueError("collect_bits measures the per-channel error tables of -sm collect: it needs %s"
                                  % ", ".join(missing))
         bap_mse = getattr(args, "bit_alloc_prior", None) == "mse"
         if bap_mse and (args.kld_threshold or args.clipping == "mix"):
-            raise NotImplementedError("-bap mse allocates from tables measured under -c laplace, gaus, no or mse, not %s"
-                                      % ("-kld" if args.kld_threshold else "-c " + args.clipping))
+            raise NotImplementedError("-bap mse allocates from tables measured under -c %s, not %s"
+                                      % (", ".join(BIT_RULES), "-kld" if args.kld_threshold else "-c " + args.clipping))
         if bap_mse and getattr(args, "mid_thread_quant", False):
             raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
         if bap_mse and args.bit_alloc_act and self.stats_mode == "no":

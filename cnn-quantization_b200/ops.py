@@ -592,10 +592,30 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
     tensor, read in place; other per-channel tensors are read as NCHW (copied when not contiguous).  Deterministic, no
     host synchronisation; with ``want_params`` also returns the [groups, 3, 6] candidate parameters (delta, offset, bits,
     scale, zero point, qmax).  Recorded in the launch profile under mode 'E' (one read of the tensor)."""
+    x, table, _, (outer, groups, inner), solve_f64, out, params = _clip_io(
+        "clip_error", x, table, layout, channels_last, solve_f64, want_params, 3, sums=3)
+    if x.numel():
+        lib = L.load()
+        ws = _own_workspace(x.device, lib.fqb200_clip_error_workspace_bytes(outer, groups, inner, int(bool(channels_last))))
+        _launch(x.device, _Timed("E", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_error,
+                x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits),
+                int(bool(positive)), int(bool(bit_alloc)), int(bool(solve_f64)), out.data_ptr(), _ptr(params),
+                ws.data_ptr(), ws.numel(), int(max_ctas))
+    return (out, params) if want_params else out
+
+
+def _clip_io(name, x, table, layout, channels_last, solve_f64, want_params, candidates, multipliers=None, bad_prior=None,
+             sums=1):
+    """The checks and outputs of clip_error, clip_mse and clip_mse_grid: (x in the memory order the launch reads, table,
+    float32 device ``multipliers`` or None, layout, ``solve_f64`` (default: one group), float64 [groups, 1 + n * ``sums``]
+    output, zero for an empty x, and [groups, n, 6] parameters or None), n = ``candidates`` (per multiplier when given).
+    ``bad_prior``, when not false, is the ValueError of an unusable prior."""
     _require_cuda_f32(x, "tensor")
     outer, groups, inner = (int(v) for v in layout)
     if outer * groups * inner != x.numel():
         raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
+    if bad_prior:
+        raise ValueError(bad_prior)
     if channels_last:
         if not cl_eligible(x, layout):
             raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
@@ -604,21 +624,17 @@ def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=Fa
     if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
             or tuple(table.shape) != (groups, L.STATS_STRIDE)):
         raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
-    table = table.contiguous()
-    lib = L.load()
-    dev = x.device
-    if solve_f64 is None:
-        solve_f64 = groups == 1
-    out = torch.empty((groups, 10), dtype=torch.float64, device=dev)
-    params = torch.empty((groups, 3, 6), dtype=torch.float32, device=dev) if want_params else None
+    mult = None
+    if multipliers is not None:
+        mult = torch.as_tensor(multipliers, dtype=torch.float32).reshape(-1).to(x.device).contiguous()
+        if not 1 <= mult.numel() <= 256:
+            raise ValueError("%s takes 1..256 multipliers, got %d" % (name, mult.numel()))
+        candidates *= mult.numel()
+    out = torch.empty((groups, 1 + candidates * sums), dtype=torch.float64, device=x.device)
     if x.numel() == 0:
         out.zero_()
-        return (out, params) if want_params else out
-    ws = _own_workspace(dev, lib.fqb200_clip_error_workspace_bytes(outer, groups, inner, int(bool(channels_last))))
-    _launch(dev, _Timed("E", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_error, x.data_ptr(), outer,
-            groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), int(bool(bit_alloc)),
-            int(bool(solve_f64)), out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
-    return (out, params) if want_params else out
+    params = torch.empty((groups, candidates, 6), dtype=torch.float32, device=x.device) if want_params else None
+    return x, table.contiguous(), mult, (outer, groups, inner), groups == 1 if solve_f64 is None else solve_f64, out, params
 
 
 CLIP_MSE_PRIORS = {"laplace": 0, "gaus": 1, "minmax": 2}
@@ -637,56 +653,26 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
     ``want_params`` also returns the [groups, K, 6] candidate parameters (delta, offset, bits, scale, zero point, qmax).
     Recorded in the launch profile under mode 'R' (one read of the tensor)."""
     bad_prior = prior not in CLIP_MSE_PRIORS or (prior == "minmax" and widths is None)
-    x, table, mult, (outer, groups, inner) = _clip_mse_inputs(
-        "clip_mse", x, table, layout, channels_last, multipliers,
+    x, table, mult, (outer, groups, inner), solve_f64, out, params = _clip_io(
+        "clip_mse", x, table, layout, channels_last, solve_f64, want_params, 1, multipliers,
         bad_prior and "prior must be one of %s (minmax with widths only), got %r" % (sorted(CLIP_MSE_PRIORS), prior))
     k = mult.numel()
     if widths is not None:
         widths = np.ascontiguousarray(widths, dtype=np.int32).reshape(-1)   # host values, validated by the library
         if widths.size != k:
             raise ValueError("clip_mse: %d widths for %d multipliers" % (widths.size, k))
-    lib = L.load()
-    dev = x.device
-    if solve_f64 is None:
-        solve_f64 = groups == 1
-    out = torch.empty((groups, k + 1), dtype=torch.float64, device=dev)
-    params = torch.empty((groups, k, 6), dtype=torch.float32, device=dev) if want_params else None
-    if x.numel() == 0:
-        out.zero_()
-        return (out, params) if want_params else out
-    ws = _own_workspace(dev, lib.fqb200_clip_mse_workspace_bytes(outer, groups, inner, int(bool(channels_last)), k))
-    head = (x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)),
-            int(bool(bit_alloc)), int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr())
-    tail = (k, out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
-    timed = _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner))
-    if widths is None:
-        _launch(dev, timed, lib.fqb200_clip_mse, *head, *tail)
-    else:
-        _launch(dev, timed, lib.fqb200_clip_mse_widths, *head, widths.ctypes.data, *tail)
+    if x.numel():
+        lib = L.load()
+        ws = _own_workspace(x.device, lib.fqb200_clip_mse_workspace_bytes(outer, groups, inner, int(bool(channels_last)), k))
+        head = (x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits),
+                int(bool(positive)), int(bool(bit_alloc)), int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr())
+        tail = (k, out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
+        timed = _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner))
+        if widths is None:
+            _launch(x.device, timed, lib.fqb200_clip_mse, *head, *tail)
+        else:
+            _launch(x.device, timed, lib.fqb200_clip_mse_widths, *head, widths.ctypes.data, *tail)
     return (out, params) if want_params else out
-
-
-def _clip_mse_inputs(name, x, table, layout, channels_last, multipliers, bad_prior):
-    """(x in the memory order the launch reads, contiguous table, float32 device multipliers, layout) of clip_mse and
-    clip_mse_grid, after their common checks; ``bad_prior``, when not false, is the ValueError of an unusable prior."""
-    _require_cuda_f32(x, "tensor")
-    outer, groups, inner = (int(v) for v in layout)
-    if outer * groups * inner != x.numel():
-        raise ValueError("layout %r does not cover %d elements" % (layout, x.numel()))
-    if bad_prior:
-        raise ValueError(bad_prior)
-    if channels_last:
-        if not cl_eligible(x, layout):
-            raise ValueError("channels_last=True needs a channels-last activation that cl_eligible takes, with layout (N, C, H*W)")
-    elif not (outer == 1 and groups == 1 and dense(x)):
-        x = x.contiguous()   # one group: any dense memory order; per channel: NCHW order
-    if (not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.device != x.device
-            or tuple(table.shape) != (groups, L.STATS_STRIDE)):
-        raise ValueError("table must be the float32 [%d, %d] statistics table on the tensor's device" % (groups, L.STATS_STRIDE))
-    mult = torch.as_tensor(multipliers, dtype=torch.float32).reshape(-1).to(x.device).contiguous()
-    if not 1 <= mult.numel() <= 256:
-        raise ValueError("%s takes 1..256 multipliers, got %d" % (name, mult.numel()))
-    return x, table.contiguous(), mult, (outer, groups, inner)
 
 
 def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multipliers, widths, prior="laplace", solve_f64=None,
@@ -697,29 +683,21 @@ def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multiplie
     multipliers[k]) - bit for bit ``clip_mse(..., [multipliers[k]], widths=[widths[i]])``.  ``prior`` "laplace" or "gaus"
     (min/max ignores the multipliers); the other arguments as in ``clip_mse``.  With ``want_params`` also returns the
     [groups, W * M, 6] candidate parameters.  Recorded in the launch profile under mode 'R'."""
-    x, table, mult, (outer, groups, inner) = _clip_mse_inputs(
-        "clip_mse_grid", x, table, layout, channels_last, multipliers,
-        prior not in ("laplace", "gaus") and "clip_mse_grid: prior must be 'laplace' or 'gaus', got %r" % (prior,))
-    m = mult.numel()
     widths = np.ascontiguousarray(widths, dtype=np.int32).reshape(-1)   # host values, validated by the library
+    x, table, mult, (outer, groups, inner), solve_f64, out, params = _clip_io(
+        "clip_mse_grid", x, table, layout, channels_last, solve_f64, want_params, widths.size, multipliers,
+        prior not in ("laplace", "gaus") and "clip_mse_grid: prior must be 'laplace' or 'gaus', got %r" % (prior,))
     if not 1 <= widths.size <= 9:
         raise ValueError("clip_mse_grid takes 1..9 widths, got %d" % widths.size)
-    n = widths.size * m
-    lib = L.load()
-    dev = x.device
-    if solve_f64 is None:
-        solve_f64 = groups == 1
-    out = torch.empty((groups, n + 1), dtype=torch.float64, device=dev)
-    params = torch.empty((groups, n, 6), dtype=torch.float32, device=dev) if want_params else None
-    if x.numel() == 0:
-        out.zero_()
-        return (out, params) if want_params else out
-    ws = _own_workspace(dev, lib.fqb200_clip_mse_grid_workspace_bytes(outer, groups, inner, int(bool(channels_last)), m,
-                                                                      widths.size))
-    _launch(dev, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse_grid, x.data_ptr(),
-            outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)), 0,
-            int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), m, widths.ctypes.data, widths.size,
-            out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
+    if x.numel():
+        lib = L.load()
+        m = mult.numel()
+        ws = _own_workspace(x.device, lib.fqb200_clip_mse_grid_workspace_bytes(outer, groups, inner, int(bool(channels_last)),
+                                                                               m, widths.size))
+        _launch(x.device, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse_grid,
+                x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits),
+                int(bool(positive)), 0, int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), m,
+                widths.ctypes.data, widths.size, out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
     return (out, params) if want_params else out
 
 

@@ -82,6 +82,13 @@ def default_base_dir():
     return os.environ.get("FQB200_STATS_DIR") or os.path.join(os.path.expanduser("~"), "mxt-sim")
 
 
+def _fresh_folder(folder):
+    """Create ``folder`` empty: a collect run replaces the files of an earlier one."""
+    if os.path.exists(folder):
+        shutil.rmtree(folder)
+    os.makedirs(folder)
+
+
 def sorted_nicely(keys):
     """Natural sort (conv2 before conv10), utils/misc.py:77-88."""
     conv = lambda t: int(t) if t.isdigit() else t
@@ -98,31 +105,39 @@ ClipErrConfig = collections.namedtuple("ClipErrConfig", "num_bits positive per_c
                                                         "bit_alloc_round bit_alloc_target")
 
 
+def _stats_table(t, cfg, channels_last):
+    """(``t`` in the memory order the launches read, layout, channels-last flag, table) of the statistics-only launch of
+    the quantizer ``cfg`` describes: per channel (with ``cfg``'s bit allocation) in place on a channels-last ``t`` when
+    ``channels_last`` allows it, else on the NCHW tensor; per tensor in any dense memory order."""
+    if not cfg.per_channel:
+        if not ops.dense(t):
+            t = t.contiguous()
+        layout = (1, 1, t.numel())
+        return t, layout, False, ops.fused(t, layout, stats_only=True, any_dense_format=True)
+    n, c = t.shape[0], t.shape[1]
+    layout = (n, c, t.numel() // (n * c))
+    cl = channels_last and ops.cl_eligible(t, layout)
+    if not cl:
+        t = t.contiguous()
+    return t, layout, cl, ops.fused(t, layout, num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
+                                    bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
+                                    bit_alloc_target=cfg.bit_alloc_target, stats_only=True, channels_last=cl)
+
+
 def _clip_sums(t, cfg, per_sample_channel):
     """float64 ops.clip_error sums (columns as there) of the contiguous ``t`` for the candidates ``cfg`` describes:
     [1, 10] over the whole tensor, or with ``per_sample_channel`` [N, C, 10] per (sample, channel) - the per-channel
     manager needs the per-sample norms of the reference's cos_sim(dims=[-1, 0]).  The candidates' statistics are those
-    of the on-the-fly launch of that quantizer (per tensor: the whole tensor; per channel: each channel, with the bit
-    allocation's widths); a per-(sample, channel) launch gets that table repeated for every group."""
-    n = t.shape[0]
-    if cfg.per_channel:
-        c = t.shape[1]
-        hw = t.numel() // (n * c)
-        table = ops.fused(t, (n, c, hw), num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
-                          bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
-                          bit_alloc_target=cfg.bit_alloc_target, stats_only=True)
-    else:
-        table = ops.fused(t, (1, 1, t.numel()), stats_only=True)
-    if not per_sample_channel:
-        if cfg.per_channel:   # all channels' errors together (a per-channel quantizer with per-tensor statistics)
-            return _clip_sums(t, cfg, True).sum((0, 1)).view(1, -1)
-        return ops.clip_error(t, table, (1, 1, t.numel()), False, cfg.num_bits, cfg.positive, solve_f64=True)
-    c = t.shape[1]
-    hw = t.numel() // (n * c)
+    of the on-the-fly launch of that quantizer (``_stats_table``); a per-(sample, channel) launch gets that table
+    repeated for every group, and a per-channel quantizer's errors over the whole tensor are the sum of its groups'."""
+    t, layout, _, table = _stats_table(t, cfg, False)
+    if not (per_sample_channel or cfg.per_channel):
+        return ops.clip_error(t, table, layout, False, cfg.num_bits, cfg.positive, solve_f64=True)
+    n, c = t.shape[0], t.shape[1]
     table = table.repeat(n, 1) if cfg.per_channel else table.expand(n * c, -1).contiguous()
-    sums = ops.clip_error(t, table, (1, n * c, hw), False, cfg.num_bits, cfg.positive, bit_alloc=cfg.bit_alloc,
-                          solve_f64=not cfg.per_channel)
-    return sums.view(n, c, 10)
+    sums = ops.clip_error(t, table, (1, n * c, t.numel() // (n * c)), False, cfg.num_bits, cfg.positive,
+                          bit_alloc=cfg.bit_alloc, solve_f64=not cfg.per_channel).view(n, c, 10)
+    return sums if per_sample_channel else sums.sum((0, 1)).view(1, -1)
 
 
 def _clip_errors(sums, count, per_channel):
@@ -223,9 +238,7 @@ class StatisticManager(object):
         if not self.save_stats:
             return
         import pandas as pd
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
+        _fresh_folder(self.folder)
         frames = {}
         for s_id, data in self.stats.items():
             df = pd.DataFrame(columns=self.stats_names, data=data)
@@ -315,9 +328,7 @@ class StatisticManagerPerChannel(object):
         if not self.save_stats:
             return
         import pandas as pd
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
+        _fresh_folder(self.folder)
         cols = []
         for c in self.stats_names:
             cols += ["min_%s" % c, "mean_%s" % c, "max_%s" % c]
@@ -373,9 +384,7 @@ class MeasureStatistics(object):
         dev = per_id[0].device
         # one device-to-host copy for all ids; float32 like the reference's values, written as its float64 column dtype
         table = torch.stack([c.to(dev) for c in per_id]).float().cpu().numpy().astype(np.float64)
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
+        _fresh_folder(self.folder)
         pd.DataFrame(data=table.T, columns=cols).to_csv(os.path.join(self.folder, "distance.csv"), index=False)
         self.stats = {}
 
@@ -431,9 +440,7 @@ class AngleStatistics(object):
         for id, mats in self.stats.items():   # one device-to-host copy per id
             out[id] = pd.DataFrame(data=torch.cat(mats).cpu().numpy().astype(np.float64))
         out["target"] = self.targets
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
+        _fresh_folder(self.folder)
         with open(os.path.join(self.folder, "angle.pkl"), "wb") as f:
             pickle.dump(out, f)
         self.stats = {}
@@ -546,28 +553,13 @@ class NoiseStatistics(object):
             n = [c[0].shape[0] for c in calls]
             tables[id] = noise_columns(yq, xs, ws, np.repeat([c[2] for c in calls], n), np.repeat([c[3] for c in calls], n),
                                        w_size, c_out)
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
+        _fresh_folder(self.folder)
         for id, table in tables.items():
             pd.DataFrame(columns=NOISE_COLUMNS, data=table).to_csv(os.path.join(self.folder, "%s.csv" % id), index=False)
         self.stats, self.weights = {}, {}
 
 
 MSE_MULTIPLIERS = tuple(0.5 + 0.125 * k for k in range(125))   # clipping values 0.5 .. 16 times b (or std)
-
-
-def _clip_table(t, cfg, channels_last):
-    """(layout, stats table) of the on-the-fly launch of the quantizer ``cfg`` describes on ``t``: per channel (with
-    the bit allocation's widths) or over the whole tensor."""
-    if not cfg.per_channel:
-        layout = (1, 1, t.numel())
-        return layout, ops.fused(t, layout, stats_only=True, any_dense_format=True)
-    n, c = t.shape[0], t.shape[1]
-    layout = (n, c, t.numel() // (n * c))
-    return layout, ops.fused(t, layout, num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
-                             bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
-                             bit_alloc_target=cfg.bit_alloc_target, stats_only=True, channels_last=channels_last)
 
 
 def best_columns(multipliers, mse):
@@ -584,7 +576,96 @@ def best_multipliers(multipliers, mse):
     return np.asarray(multipliers, dtype=np.float32)[best_columns(multipliers, mse)]
 
 
-class ClipMseStatistics(object):
+def _mse_multipliers(multipliers, prior):
+    """float32 ``multipliers`` (default MSE_MULTIPLIERS) of the clipping values alpha = m * b (``prior`` "laplace") or
+    m * std ("gaus"), after checking both."""
+    if prior not in ("gaus", "laplace"):
+        raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
+    m = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers, dtype=np.float32).reshape(-1)
+    if not 1 <= m.size <= 256:
+        raise ValueError("mse_multipliers: 1..256 values, got %d" % m.size)
+    return m
+
+
+class _CallSiteSums(object):
+    """The collect and use halves ClipMseStatistics and BitMseStatistics share: per call site, device sums of one launch
+    per batch (``_add``), which ``__exit__`` reads back in one copy and writes as ``_tables`` makes them; with ``load``,
+    the pickle, read on first use (``_entry``).  Errors name the collect flag FLAG and the use-mode option USE."""
+
+    def __init__(self, folder, base_dir, load):
+        self.folder = os.path.join(base_dir or default_base_dir(), self.KIND, folder)
+        self.load = load
+        self.acc = {}    # id -> (sums [G, n], scales [G, s], float64 device tensors, batches)
+        self.meta = {}   # id -> (internal_name, what _tables needs of the call site, elements per group and batch)
+        self._mult_dev = {}
+        self._loaded = None
+
+    @property
+    def path(self):
+        return os.path.join(self.folder, self.FILE)
+
+    # -- collect ---------------------------------------------------------------------------------------------------
+    def _device_multipliers(self, values, device, *key):
+        """``values`` as a float32 tensor on ``device``, made once per (device, ``key``)."""
+        mult = self._mult_dev.get((device,) + key)
+        if mult is None:
+            mult = self._mult_dev[(device,) + key] = torch.from_numpy(np.asarray(values, dtype=np.float32)).to(device)
+        return mult
+
+    def _add(self, id, sums, scales, meta):
+        prev = self.acc.get(id)
+        if prev is None:
+            self.acc[id] = (sums, scales, 1)
+            self.meta[id] = meta
+            return
+        if prev[0].shape != sums.shape:
+            raise ValueError("%s of %r: %d %s in this call, %d before" % (self.FLAG, id, sums.shape[0], self.GROUPS,
+                                                                          prev[0].shape[0]))
+        self.acc[id] = (prev[0] + sums, prev[1] + scales, prev[2] + 1)
+
+    def _read_back(self):
+        """(id, sums, batch-mean scales, element count per group, internal name, meta) per call site, from one copy."""
+        flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
+        pos = 0
+        for id, (sums, scales, batches) in self.acc.items():
+            g, n = sums.shape
+            s = flat[pos:pos + g * n].reshape(g, n)
+            pos += g * n
+            k = scales.shape[1]
+            sc = flat[pos:pos + g * k].reshape(g, k) / batches
+            pos += g * k
+            tag, info, per_batch = self.meta[id]
+            yield id, s, sc, np.full(g, float(per_batch * batches)), tag, info
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *args):
+        if self.load or not self.acc:
+            return
+        out, csv = self._tables(self._read_back())
+        _fresh_folder(self.folder)
+        with open(self.path, "wb") as f:
+            pickle.dump(out, f)
+        csv.to_csv(os.path.join(self.folder, self.CSV), index=False)
+        self.acc, self.meta = {}, {}
+
+    # -- use -------------------------------------------------------------------------------------------------------
+    def _entry(self, id):
+        """The pickle's DataFrame of ``id`` (the pickle is read on first use); KeyError naming FLAG when there is none."""
+        if self._loaded is None:
+            if not os.path.exists(self.path):
+                raise KeyError("%s needs the %ss at %s: collect them with %s=True" % (self.USE, self.WHAT, self.path,
+                                                                                      self.FLAG))
+            with open(self.path, "rb") as f:
+                self._loaded = pickle.load(f)
+        df = self._loaded.get(id)
+        if df is None:
+            raise KeyError("%s needs the %s of layer %r: collect it with %s=True" % (self.USE, self.WHAT, id, self.FLAG))
+        return df
+
+
+class ClipMseStatistics(_CallSiteSums):
     """Clipping-MSE curves (`collect_mse`): ``save_curve(t, tag, id, cfg)`` adds, per group of the quantizer ``cfg`` (a
     ClipErrConfig, as collect_err passes) describes, the float64 sums of ops.clip_mse over ``multipliers`` (alpha = m * b
     with prior "laplace", m * std with "gaus") and the group's b, std and width to device accumulators; ``__exit__``
@@ -593,76 +674,36 @@ class ClipMseStatistics(object):
     curve.csv holds layer totals per element: mse = sum_g sum (x - q)^2 / sum_g count, and the reference's analytic
     curves (mse_analysis.py) per group at the same alpha, with that group's b or std and width (width + 1 for a positive
     range, the relation the reference's *_positive ACIQ tables encode), weighted by the group's count."""
+    KIND, FILE, CSV = "clip_mse", "clip_mse.pkl", "curve.csv"
+    FLAG, USE, WHAT, GROUPS = "collect_mse", "-c mse", "clipping-MSE curve", "groups"
 
     def __init__(self, folder, multipliers=None, prior="laplace", base_dir=None, load=False):
-        if prior not in ("gaus", "laplace"):
-            raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
-        self.folder = os.path.join(base_dir or default_base_dir(), "clip_mse", folder)
-        self.multipliers = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers, dtype=np.float32).reshape(-1)
-        if not 1 <= self.multipliers.size <= 256:
-            raise ValueError("mse_multipliers: 1..256 values, got %d" % self.multipliers.size)
+        self.multipliers = _mse_multipliers(multipliers, prior)
         self.prior = prior
-        self.load = load
-        self.curves = None
-        self.acc = {}    # id -> (sums [G, K + 1], b / std / bits sums [G, 3], float64 device tensors, batches)
-        self.meta = {}   # id -> (internal_name, positive, elements per group and batch)
-        self._mult_dev = {}
+        super(ClipMseStatistics, self).__init__(folder, base_dir, load)
 
     # -- collect ---------------------------------------------------------------------------------------------------
     def save_curve(self, tensor, tag, id, cfg):
-        t = tensor.detach()
-        if cfg.per_channel:
-            n, c = t.shape[0], t.shape[1]
-            cl = ops.cl_eligible(t, (n, c, t.numel() // (n * c)))
-        else:
-            cl = False
-        if not (cl or (ops.dense(t) and not cfg.per_channel)):
-            t = t.contiguous()   # per channel: NCHW order; one group: any dense memory order
-        layout, table = _clip_table(t, cfg, cl)
-        mult = self._mult_dev.get(t.device)
-        if mult is None:
-            mult = self._mult_dev[t.device] = torch.from_numpy(self.multipliers).to(t.device)
-        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=self.prior,
+        t, layout, cl, table = _stats_table(tensor.detach(), cfg, True)
+        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive,
+                            self._device_multipliers(self.multipliers, t.device), prior=self.prior,
                             bit_alloc=cfg.bit_alloc, solve_f64=not cfg.per_channel)
         bits = table[:, 7] if cfg.bit_alloc else torch.full_like(table[:, 7], float(cfg.num_bits))
-        scales = torch.stack([table[:, 3], table[:, 4], bits], 1).double()
-        prev = self.acc.get(id)
-        if prev is None:
-            self.acc[id] = (sums, scales, 1)
-            self.meta[id] = (tag, bool(cfg.positive), layout[0] * layout[2])
-        else:
-            if prev[0].shape != sums.shape:
-                raise ValueError("collect_mse of %r: %d groups in this call, %d before" % (id, sums.shape[0], prev[0].shape[0]))
-            self.acc[id] = (prev[0] + sums, prev[1] + scales, prev[2] + 1)
+        self._add(id, sums, torch.stack([table[:, 3], table[:, 4], bits], 1).double(),
+                  (tag, bool(cfg.positive), layout[0] * layout[2]))
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *args):
-        if self.load or not self.acc:
-            return
+    def _tables(self, groups):
         import pandas as pd
         from . import mse_analysis
-        ids = list(self.acc)
-        flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
         k = self.multipliers.size
         mults = self.multipliers.astype(np.float64)
         out = {"multipliers": mults, "prior": self.prior}
         rows = []
-        pos = 0
-        for id in ids:
-            sums, scales, batches = self.acc[id]
-            g = sums.shape[0]
-            s = flat[pos:pos + g * (k + 1)].reshape(g, k + 1)
-            pos += g * (k + 1)
-            sc = flat[pos:pos + g * 3].reshape(g, 3) / batches
-            pos += g * 3
-            tag, positive, per_batch = self.meta[id]
-            count = np.full(g, float(per_batch * batches))
+        for id, s, sc, count, tag, positive in groups:
+            g = s.shape[0]
             mse = s[:, 1:] / count[:, None]
             df = pd.DataFrame({"count": count, "b": sc[:, 0], "std": sc[:, 1], "bits": sc[:, 2]})
-            df = pd.concat([df, pd.DataFrame(mse, columns=["mse_%d" % j for j in range(k)])], axis=1)
-            out[id] = df
+            out[id] = pd.concat([df, pd.DataFrame(mse, columns=["mse_%d" % j for j in range(k)])], axis=1)
             width = sc[:, 2] + (1 if positive else 0)
             scale = sc[:, 0] if self.prior == "laplace" else sc[:, 1]
             lap = np.empty((g, k))
@@ -678,32 +719,20 @@ class ClipMseStatistics(object):
                 gau_t = (count[:, None] * gau).sum(0) / total
             for j in range(k):
                 rows.append((id, tag, mults[j], layer[j], lap_t[j], gau_t[j]))
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
-        with open(os.path.join(self.folder, "clip_mse.pkl"), "wb") as f:
-            pickle.dump(out, f)
-        pd.DataFrame(rows, columns=["id", "internal_name", "multiplier", "mse", "mse_laplace_analytic",
-                                    "mse_gaus_analytic"]).to_csv(os.path.join(self.folder, "curve.csv"), index=False)
-        self.acc, self.meta = {}, {}
+        return out, pd.DataFrame(rows, columns=["id", "internal_name", "multiplier", "mse", "mse_laplace_analytic",
+                                                "mse_gaus_analytic"])
 
     # -- use (`-c mse`) ----------------------------------------------------------------------------------------------
     def best(self, id):
         """(m* per group as float32 [G], prior) of the curve collected for ``id``; KeyError naming collect_mse when there
         is none."""
-        if self.curves is None:
-            path = os.path.join(self.folder, "clip_mse.pkl")
-            if not os.path.exists(path):
-                raise KeyError("-c mse needs the clipping-MSE curves at %s: collect them with collect_mse=True" % path)
-            with open(path, "rb") as f:
-                self.curves = pickle.load(f)
-        df = self.curves.get(id)
-        if df is None:
-            raise KeyError("-c mse needs the clipping-MSE curve of layer %r: collect it with collect_mse=True" % (id,))
-        m = self.curves["multipliers"]
-        return best_multipliers(m, df[["mse_%d" % j for j in range(len(m))]].to_numpy()), self.curves["prior"]
+        df = self._entry(id)
+        m = self._loaded["multipliers"]
+        return best_multipliers(m, df[["mse_%d" % j for j in range(len(m))]].to_numpy()), self._loaded["prior"]
 
 
+# The clipping rules a bit-allocation table is measured under (`collect_bits`) and `-bap mse` allocates from: the first
+# three with the width candidates of ``bit_candidates``; "mse" (`-c mse`) over a grid of widths and multipliers.
 BIT_RULES = ("laplace", "gaus", "no", "mse")
 
 
@@ -723,7 +752,7 @@ def bit_candidates(rule, positive, num_bits):
     raise ValueError("bit allocation tables are measured under clipping %s, got %r" % (list(BIT_RULES[:3]), rule))
 
 
-class BitMseStatistics(object):
+class BitMseStatistics(_CallSiteSums):
     """Per-channel error tables of bit allocation (`collect_bits`): ``save_table(t, tag, id, cfg)`` adds, for a call site
     whose quantizer ``cfg`` (a ClipErrConfig) quantizes per channel with bit allocation, the float64 sums of one
     ops.clip_mse launch over the 9 candidates of ``bit_candidates(rule, ...)`` and the channels' b and std to device
@@ -731,87 +760,47 @@ class BitMseStatistics(object):
     one ops.clip_mse_grid over widths 0..8 times ``multipliers`` (alpha = m * b with ``prior`` "laplace", m * std with
     "gaus"), and each width's error is the one at its best multiplier (``best_columns``).  ``__exit__`` writes bit_mse.pkl
     and alloc.csv.  With ``load`` the instance reads bit_mse.pkl instead (on first use), for `-bap mse`."""
+    KIND, FILE, CSV = "bit_mse", "bit_mse.pkl", "alloc.csv"
+    FLAG, USE, WHAT, GROUPS = "collect_bits", "-bap mse", "per-channel error table", "channels"
 
     def __init__(self, folder, rule=None, base_dir=None, load=False, multipliers=None, prior="laplace"):
         if not load and rule not in BIT_RULES:
             raise ValueError("collect_bits measures under clipping %s, got %r" % (list(BIT_RULES), rule))
-        self.folder = os.path.join(base_dir or default_base_dir(), "bit_mse", folder)
         self.rule = rule
         if rule == "mse":
-            if prior not in ("gaus", "laplace"):
-                raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
-            self.multipliers = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers,
-                                          dtype=np.float32).reshape(-1)
-            if not 1 <= self.multipliers.size <= 256:
-                raise ValueError("mse_multipliers: 1..256 values, got %d" % self.multipliers.size)
+            self.multipliers = _mse_multipliers(multipliers, prior)
             self.prior = prior
-        self.load = load
-        self.tables = None
-        self.acc = {}    # id -> (sums [G, 10] or, rule "mse", [G, 1 + 9 M], b / std sums [G, 2], float64 device tensors, batches)
-        self.meta = {}   # id -> (internal_name, ClipErrConfig, elements per channel and batch)
-        self._mult_dev = {}
+        super(BitMseStatistics, self).__init__(folder, base_dir, load)
 
     # -- collect ---------------------------------------------------------------------------------------------------
     def save_table(self, tensor, tag, id, cfg):
         if not (cfg.per_channel and cfg.bit_alloc):
             return
-        t = tensor.detach()
-        n, c = t.shape[0], t.shape[1]
-        layout = (n, c, t.numel() // (n * c))
-        cl = ops.cl_eligible(t, layout)
-        if not cl:
-            t = t.contiguous()
-        table = ops.fused(t, layout, num_bits=8, stats_only=True, channels_last=cl)
+        # an 8-bit table without allocation: every candidate brings its own width
+        t, layout, cl, table = _stats_table(tensor.detach(), cfg._replace(bit_alloc=False), True)
         if self.rule == "mse":
-            mult = self._mult_dev.get(t.device)
-            if mult is None:
-                mult = self._mult_dev[t.device] = torch.from_numpy(self.multipliers).to(t.device)
-            sums = ops.clip_mse_grid(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, range(9), prior=self.prior,
+            sums = ops.clip_mse_grid(t, table, layout, cl, cfg.num_bits, cfg.positive,
+                                     self._device_multipliers(self.multipliers, t.device), range(9), prior=self.prior,
                                      solve_f64=False)
         else:
             mults, prior = bit_candidates(self.rule, cfg.positive, cfg.num_bits)
-            key = (t.device, bool(cfg.positive), cfg.num_bits)
-            mult = self._mult_dev.get(key)
-            if mult is None:
-                mult = self._mult_dev[key] = torch.tensor(mults, dtype=torch.float32, device=t.device)
-            sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, mult, prior=prior, widths=range(9),
-                                solve_f64=False)
-        scales = table[:, 3:5].double()
-        prev = self.acc.get(id)
-        if prev is None:
-            self.acc[id] = (sums, scales, 1)
-            self.meta[id] = (tag, cfg, layout[0] * layout[2])
-        else:
-            if prev[0].shape != sums.shape:
-                raise ValueError("collect_bits of %r: %d channels in this call, %d before" % (id, sums.shape[0], prev[0].shape[0]))
-            self.acc[id] = (prev[0] + sums, prev[1] + scales, prev[2] + 1)
+            sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive,
+                                self._device_multipliers(mults, t.device, bool(cfg.positive), cfg.num_bits), prior=prior,
+                                widths=range(9), solve_f64=False)
+        self._add(id, sums, table[:, 3:5].double(), (tag, cfg, layout[0] * layout[2]))
 
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *args):
-        if self.load or not self.acc:
-            return
+    def _tables(self, groups):
         import pandas as pd
         from . import _lib as L
         from .bit_alloc import allocate
         from .int_quantizer import IntQuantizer
-        flat = torch.cat([torch.cat([a[0].reshape(-1), a[1].reshape(-1)]) for a in self.acc.values()]).cpu().numpy()
         out = {"rule": self.rule}
         joint = self.rule == "mse"
         if joint:
             out.update(multipliers=self.multipliers.astype(np.float64), prior=self.prior)
         rows = []
-        pos = 0
-        for id in list(self.acc):
-            sums, _, batches = self.acc[id]
-            g, n = sums.shape
-            s = flat[pos:pos + g * n].reshape(g, n)
-            pos += g * n
-            sc = flat[pos:pos + g * 2].reshape(g, 2) / batches
-            pos += g * 2
-            tag, cfg, per_batch = self.meta[id]
-            count = np.full(g, float(per_batch * batches))
+        for id, s, sc, count, tag, cfg in groups:
+            g = s.shape[0]
             df = pd.DataFrame({"count": count, "b": sc[:, 0], "std": sc[:, 1], "positive": np.full(g, bool(cfg.positive))})
             if joint:   # each width's sum at its best multiplier
                 grid = s[:, 1:].reshape(g, 9, -1)
@@ -832,37 +821,19 @@ class BitMseStatistics(object):
             for w in allocations:
                 row += [int(w.sum()), float(sse[np.arange(g), w].sum() / count.sum())]
             rows.append(row)
-        if os.path.exists(self.folder):
-            shutil.rmtree(self.folder)
-        os.makedirs(self.folder)
-        with open(self.path, "wb") as f:
-            pickle.dump(out, f)
-        pd.DataFrame(rows, columns=ALLOC_COLUMNS).to_csv(os.path.join(self.folder, "alloc.csv"), index=False)
-        self.acc, self.meta = {}, {}
+        return out, pd.DataFrame(rows, columns=ALLOC_COLUMNS)
 
     # -- use (`-bap mse`) --------------------------------------------------------------------------------------------
-    @property
-    def path(self):
-        return os.path.join(self.folder, "bit_mse.pkl")
-
     def table(self, id):
         """(float64 [C, 9] per-element MSE of widths 0..8, rule) collected for ``id``; KeyError naming collect_bits when
         there is none."""
-        if self.tables is None:
-            if not os.path.exists(self.path):
-                raise KeyError("-bap mse needs the per-channel error tables at %s: collect them with collect_bits=True"
-                               % self.path)
-            with open(self.path, "rb") as f:
-                self.tables = pickle.load(f)
-        df = self.tables.get(id)
-        if df is None:
-            raise KeyError("-bap mse needs the per-channel error table of layer %r: collect it with collect_bits=True" % (id,))
-        return df[["mse_w%d" % w for w in range(9)]].to_numpy(dtype=np.float64), self.tables["rule"]
+        df = self._entry(id)
+        return df[["mse_w%d" % w for w in range(9)]].to_numpy(dtype=np.float64), self._loaded["rule"]
 
     def multipliers_of(self, id):
         """(float32 [C, 9] best multiplier of each width, prior) of a joint table (rule "mse") collected for ``id``."""
-        self.table(id)
-        return self.tables[id][["m_w%d" % w for w in range(9)]].to_numpy(dtype=np.float32), self.tables["prior"]
+        df = self._entry(id)
+        return df[["m_w%d" % w for w in range(9)]].to_numpy(dtype=np.float32), self._loaded["prior"]
 
 
 ALLOC_COLUMNS = ["id", "internal_name", "groups", "target", "bits_uniform", "mse_uniform", "bits_analytic", "mse_analytic",

@@ -255,40 +255,125 @@ def test_default_collect_writes_nan_error_columns(monkeypatch, tmp_path):
         assert df["mean_" + c].isna().all()
 
 
-@pytest.mark.parametrize("per_channel,bit_alloc", [(False, False), (True, False), (True, True)])
-def test_managers_launch_the_configured_candidates(monkeypatch, tmp_path, per_channel, bit_alloc):
-    """What reaches ops.clip_error: per tensor, one float64-solved group at the configured width and never a bit
-    allocation; per channel (per-channel manager), the (sample, channel) groups with the channel table repeated per
-    sample and the allocation's widths only when configured."""
+@pytest.mark.parametrize("per_channel,bit_alloc,channels_last", [
+    (False, False, False), (True, False, False), (True, True, False), (False, False, True), (True, False, True),
+    (True, True, True)], ids=["False-False", "True-False", "True-True", "False-False-cl", "True-False-cl", "True-True-cl"])
+def test_managers_launch_the_configured_candidates(monkeypatch, tmp_path, per_channel, bit_alloc, channels_last):
+    """What the collect measurements launch for a call site's quantizer.  collect_err (ops.clip_error): per tensor, one
+    float64-solved group at the configured width and never a bit allocation; per channel (per-channel manager), the
+    (sample, channel) groups of the NCHW tensor with the channel table repeated per sample and the allocation's widths
+    only when configured; a per-tensor manager sums the same per-channel launch and runs its statistics launch once.
+    collect_mse (ops.clip_mse) and collect_bits (ops.clip_mse or, under -c mse, ops.clip_mse_grid): per channel on a
+    channels-last tensor the kernels take in place, per tensor on any dense memory order, else on the NCHW tensor."""
     from cnn_quantization_b200 import _lib as L, ops
-    from cnn_quantization_b200.statistics import ClipErrConfig, StatisticManager, StatisticManagerPerChannel
+    from cnn_quantization_b200.statistics import (BitMseStatistics, ClipErrConfig, ClipMseStatistics, StatisticManager,
+                                                  StatisticManagerPerChannel, bit_candidates)
     launches, tables = [], []
 
-    def fused(x, layout, stats_only=False, bit_alloc=False, **kw):
+    def fused(x, layout, stats_only=False, bit_alloc=False, num_bits=8, channels_last=False, any_dense_format=False, **kw):
         t = torch.arange(int(layout[1]) * 12, dtype=torch.float32).view(-1, 12)
-        tables.append((tuple(layout), bit_alloc, t))
+        tables.append(dict(layout=tuple(layout), bit_alloc=bit_alloc, num_bits=num_bits, channels_last=channels_last,
+                           any_dense_format=any_dense_format, kw=kw, table=t))
         return t
 
     def clip_error(x, table, layout, channels_last, num_bits, positive, bit_alloc=False, solve_f64=None, **kw):
-        launches.append(dict(layout=tuple(layout), num_bits=num_bits, positive=positive, bit_alloc=bit_alloc,
-                             solve_f64=solve_f64, table=table.clone()))
+        launches.append(dict(op="clip_error", layout=tuple(layout), num_bits=num_bits, positive=positive,
+                             bit_alloc=bit_alloc, solve_f64=solve_f64, table=table.clone(), channels_last=channels_last,
+                             nhwc=ops.nhwc(x)))
         return torch.ones((int(layout[1]), 10), dtype=torch.float64)
+
+    def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, prior="laplace", bit_alloc=False,
+                 solve_f64=None, widths=None, **kw):
+        launches.append(dict(op="clip_mse", layout=tuple(layout), num_bits=num_bits, positive=positive,
+                             bit_alloc=bit_alloc, solve_f64=solve_f64, table=table, channels_last=channels_last,
+                             nhwc=ops.nhwc(x), prior=prior, multipliers=torch.as_tensor(multipliers).tolist(),
+                             widths=None if widths is None else list(widths)))
+        return torch.ones((int(layout[1]), len(launches[-1]["multipliers"]) + 1), dtype=torch.float64)
+
+    def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multipliers, widths, prior="laplace",
+                      solve_f64=None, **kw):
+        launches.append(dict(op="clip_mse_grid", layout=tuple(layout), num_bits=num_bits, positive=positive,
+                             solve_f64=solve_f64, table=table, channels_last=channels_last, nhwc=ops.nhwc(x), prior=prior,
+                             multipliers=torch.as_tensor(multipliers).tolist(), widths=list(widths)))
+        return torch.ones((int(layout[1]), 1 + 9 * len(launches[-1]["multipliers"])), dtype=torch.float64)
 
     monkeypatch.setattr(ops, "fused", fused)
     monkeypatch.setattr(ops, "clip_error", clip_error)
+    monkeypatch.setattr(ops, "clip_mse", clip_mse)
+    monkeypatch.setattr(ops, "clip_mse_grid", clip_mse_grid)
     cfg = ClipErrConfig(num_bits=4, positive=True, per_channel=per_channel, bit_alloc=bit_alloc, bit_alloc_prior=L.PRIOR_STD,
                         bit_alloc_round=True, bit_alloc_target=4)
-    x = torch.randn(2, 3, 4, 4)
+    x = torch.randn(2, 4, 4, 4)
+    if channels_last:
+        x = x.to(memory_format=torch.channels_last)
+        assert ops.cl_eligible(x)
+    chan_layout = (2, 4, 16) if per_channel else (1, 1, 128)
+    cl = per_channel and channels_last
+
+    def stats_launch(t, alloc):
+        """The statistics-only launch of the quantizer ``cfg``, with its bit allocation when ``alloc``."""
+        assert t["layout"] == chan_layout and t["bit_alloc"] == alloc and t["num_bits"] == (4 if alloc else 8)
+        if alloc:
+            assert t["kw"]["bit_alloc_prior"] == L.PRIOR_STD and t["kw"]["bit_alloc_round"] and t["kw"]["bit_alloc_target"] == 4
+        assert per_channel or t["any_dense_format"]
+
+    # -- collect_err ---------------------------------------------------------------------------------------------------------
     if not per_channel:
         StatisticManager("m", load_stats=False, base_dir=str(tmp_path)).save_tensor_stats(x, "a", "conv1_activation",
                                                                                          clip_err=cfg)
         (l,) = launches
-        assert l["layout"] == (1, 1, 96) and l["num_bits"] == 4 and l["positive"] and not l["bit_alloc"] and l["solve_f64"]
-        return
-    sm = StatisticManagerPerChannel("m", load_stats=False, collect_err=True, base_dir=str(tmp_path))
-    sm.save_tensor_stats(x, "a", "conv1_activation", clip_err=cfg)
-    (l,) = launches
-    assert l["layout"] == (1, 6, 16) and l["bit_alloc"] == bit_alloc and not l["solve_f64"]
-    chan = [t for lay, ba, t in tables if lay == (2, 3, 16) and ba == bit_alloc][-1]
-    assert torch.equal(l["table"], chan.repeat(2, 1))   # row n * C + c = channel c
-    assert set(sm.stats["conv1_activation"]) >= {"mse_lowp", "cos_laplace"}
+        assert l["layout"] == (1, 1, 128) and l["num_bits"] == 4 and l["positive"] and not l["bit_alloc"] and l["solve_f64"]
+        assert not l["channels_last"] and not l["nhwc"]
+    else:
+        sm = StatisticManagerPerChannel("m", load_stats=False, collect_err=True, base_dir=str(tmp_path))
+        sm.save_tensor_stats(x, "a", "conv1_activation", clip_err=cfg)
+        (l,) = launches
+        assert l["layout"] == (1, 8, 16) and l["bit_alloc"] == bit_alloc and not l["solve_f64"]
+        assert not l["channels_last"] and not l["nhwc"]
+        chan = [t for t in tables if t["layout"] == (2, 4, 16) and t["bit_alloc"] == bit_alloc][-1]
+        assert not chan["channels_last"]
+        assert torch.equal(l["table"], chan["table"].repeat(2, 1))   # row n * C + c = channel c
+        assert set(sm.stats["conv1_activation"]) >= {"mse_lowp", "cos_laplace"}
+        # a per-channel quantizer under the per-tensor manager: all channels' errors together, one statistics launch
+        del launches[:], tables[:]
+        StatisticManager("m", load_stats=False, base_dir=str(tmp_path)).save_tensor_stats(x, "a", "conv1_activation",
+                                                                                         clip_err=cfg)
+        (l,) = launches
+        assert l["layout"] == (1, 8, 16) and l["bit_alloc"] == bit_alloc and not l["solve_f64"] and not l["nhwc"]
+        chan = [t for t in tables if t["layout"] == (2, 4, 16)]
+        assert len(chan) == 1
+        stats_launch(chan[0], bit_alloc)
+        assert torch.equal(l["table"], chan[0]["table"].repeat(2, 1))
+
+    # -- collect_mse ---------------------------------------------------------------------------------------------------------
+    for prior in ("laplace", "gaus"):
+        del launches[:], tables[:]
+        ClipMseStatistics("m", multipliers=[1.0, 2.5, 4.0], prior=prior, base_dir=str(tmp_path)).save_curve(
+            x, "a", "conv1_activation", cfg)
+        (t,), (l,) = tables, launches
+        stats_launch(t, bit_alloc)
+        assert t["channels_last"] == cl
+        assert l["op"] == "clip_mse" and l["table"] is t["table"] and l["layout"] == chan_layout
+        assert l["channels_last"] == cl and l["nhwc"] == (channels_last and (cl or not per_channel))
+        assert l["num_bits"] == 4 and l["positive"] and l["bit_alloc"] == bit_alloc and l["solve_f64"] == (not per_channel)
+        assert l["prior"] == prior and l["multipliers"] == [1.0, 2.5, 4.0] and l["widths"] is None
+
+    # -- collect_bits --------------------------------------------------------------------------------------------------------
+    for rule in ("laplace", "gaus", "no", "mse"):
+        del launches[:], tables[:]
+        BitMseStatistics("m", rule, base_dir=str(tmp_path), multipliers=[1.0, 2.5], prior="gaus").save_table(
+            x, "a", "conv1_activation", cfg)
+        if not (per_channel and bit_alloc):
+            assert not launches and not tables
+            continue
+        (t,), (l,) = tables, launches
+        stats_launch(t, False)   # an 8-bit table without allocation: every width is a candidate of its own
+        assert t["channels_last"] == cl
+        assert l["table"] is t["table"] and l["layout"] == chan_layout and l["channels_last"] == cl and l["nhwc"] == cl
+        assert l["num_bits"] == 4 and l["positive"] and not l["solve_f64"] and l["widths"] == list(range(9))
+        if rule == "mse":
+            assert l["op"] == "clip_mse_grid" and l["prior"] == "gaus" and l["multipliers"] == [1.0, 2.5]
+        else:
+            mults, p = bit_candidates(rule, True, 4)
+            assert l["op"] == "clip_mse" and not l["bit_alloc"] and l["prior"] == p
+            assert l["multipliers"] == torch.tensor(mults, dtype=torch.float32).tolist()
