@@ -423,7 +423,7 @@ class QuantizationManagerInference(object):
         self.clip_mse = None
         # `collect_bits`: the collect hooks also measure the per-channel error tables `-bap mse` allocates from
         self.collect_bits = bool(getattr(args, "collect_bits", False))
-        from .statistics import BIT_RULES
+        from .statistics import BIT_RULES, refuse_bap_mse
         if self.collect_bits:
             missing = [what for what, ok in (("stats_mode='collect'", self.stats_mode == "collect"),
                                               ("a qtype", args.qtype is not None),
@@ -436,17 +436,11 @@ class QuantizationManagerInference(object):
                 raise ValueError("collect_bits measures the per-channel error tables of -sm collect: it needs %s"
                                  % ", ".join(missing))
         bap_mse = getattr(args, "bit_alloc_prior", None) == "mse"
-        if bap_mse and (args.kld_threshold or args.clipping == "mix"):
-            raise NotImplementedError("-bap mse allocates from tables measured under -c %s, not %s"
-                                      % (", ".join(BIT_RULES), "-kld" if args.kld_threshold else "-c " + args.clipping))
-        if bap_mse and getattr(args, "mid_thread_quant", False):
-            raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
-        if bap_mse and args.bit_alloc_act and self.stats_mode == "no":
-            raise NotImplementedError("-baa -bap mse allocates from collected tables: it needs -sm use (collect them with "
-                                      "collect_bits=True)")
-        if bap_mse and args.bit_alloc_act and (self.collect_err or self.collect_mse):
-            raise NotImplementedError("-baa -bap mse: collect_err and collect_mse would measure their candidates at the "
-                                      "analytic widths, not at the widths -bap mse runs with")
+        if bap_mse:   # a k*std rule is refused by the quantizer, at the call sites that would allocate under it
+            refuse_bap_mse(kld=args.kld_threshold, clipping="mix" if args.clipping == "mix" else None,
+                           mid_tread=getattr(args, "mid_thread_quant", False),
+                           needs_use=args.bit_alloc_act and self.stats_mode == "no",
+                           collect=args.bit_alloc_act and (self.collect_err or self.collect_mse))
         self.bit_mse = None
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None

@@ -736,6 +736,28 @@ class ClipMseStatistics(_CallSiteSums):
 BIT_RULES = ("laplace", "gaus", "no", "mse")
 
 
+def refuse_bap_mse(kld=False, clipping=None, mid_tread=False, needs_use=False, collect=False, widths_alone=False):
+    """Raise NotImplementedError where `-bap mse` would otherwise run another allocation in its place: widths under
+    ``-kld`` or a ``clipping`` rule no table is measured under (None: not asked), the ``mid_tread`` (-mtq) bins,
+    `-baa` without `-sm use` (``needs_use``), `-baa` while ``collect_err`` / ``collect_mse`` measure (``collect``), and
+    the width alone under -c mse (``widths_alone``).  The manager calls it with the run's flags, the quantizer on the
+    paths that would run the analytic rule."""
+    if widths_alone and clipping == "mse":
+        raise NotImplementedError("-bap mse under -c mse picks each channel's width together with its clipping value "
+                                  "from the joint tables, not the width alone")
+    if kld or (clipping is not None and clipping not in BIT_RULES):
+        raise NotImplementedError("-bap mse allocates from tables measured under -c %s, not %s"
+                                  % (", ".join(BIT_RULES), "-kld" if kld else "-c " + clipping))
+    if mid_tread:
+        raise NotImplementedError("-bap mse does not allocate the mid-tread (-mtq) bins")
+    if needs_use:
+        raise NotImplementedError("-baa -bap mse allocates from per-channel error tables collected with "
+                                  "collect_bits=True: it needs -sm use")
+    if collect:
+        raise NotImplementedError("-baa -bap mse: collect_err and collect_mse would measure their candidates at the "
+                                  "analytic widths, not at the widths -bap mse runs with")
+
+
 def bit_candidates(rule, positive, num_bits):
     """(multipliers, ops.clip_mse prior) of the 9 candidates of width w = 0..8: what `-sm use` runs on a channel
     allocated w bits under the clipping ``rule`` - the Laplace ACIQ factor of w on b (int_quantizer.py:236-253), the Gauss
