@@ -399,6 +399,18 @@ __device__ __noinline__ void solve_params(const FusedArgs& A, LeaderSmem& sm) {
     solve_mid_tread(A, sm);
     return;
   }
+  if (A.g_delta) {
+    // fqb200_quantize_weights_given: the caller's per-row (delta, offset, bits) stand in for the solve; the statistics
+    // phases ran only for the corrections
+    for (unsigned g = threadIdx.x; g < G; g += kThreads) {
+      const float delta = A.g_delta[g], offset = A.g_offset[g];
+      const float bits = A.g_bits ? A.g_bits[g] : static_cast<float>(A.num_bits);
+      A.lp[g] = make_leaf_param(A.leaf, delta, offset, bits);
+      A.gdelta[g] = delta;
+      A.goffset[g] = offset;
+    }
+    return;
+  }
   const bool alloc = A.bit_alloc && A.num_bits <= 4 && A.scope == FQB200_SCOPE_GROUP;
   if (alloc) solve_bit_alloc(A, sm);
   stamp(A, 12);
@@ -1106,6 +1118,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) fq_fused_kernel(const __
 #include "fq_kmeans.cuh"
 #include "fq_angle.cuh"
 #include "fq_sample_sums.cuh"
+#include "fq_alloc.cuh"
 namespace fqb {
 
 // Standalone a1 with host-side scalars (gemmlowp.cu:30-45): flat grid-stride, parameters by value.
@@ -2851,6 +2864,125 @@ int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_
   e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(fqb::kThreads), args, smem, st);
   if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch fq_kmeans_kernel: %s", cudaGetErrorString(e));
   return FQB200_OK;
+}
+
+// The descriptor of the RANGE_MINMAX weight launch whose plan fqb200_quantize_weights_given runs: bits given = that
+// launch with bit allocation (prior std), so the phases, their walking directions and the workspace are the same.
+static fqb200_desc weights_given_desc(int64_t groups, int64_t inner, int32_t num_bits, bool has_bits, int32_t bias_corr,
+                                      int32_t var_corr, unsigned long long* hist) {
+  fqb200_desc d;
+  memset(&d, 0, sizeof(d));
+  d.outer = 1;
+  d.groups = groups;
+  d.inner = inner;
+  d.scope = FQB200_SCOPE_GROUP;
+  d.range_mode = FQB200_RANGE_MINMAX;
+  d.leaf = FQB200_LEAF_TORCH;
+  d.num_bits = num_bits;
+  d.bit_alloc = has_bits ? 1 : 0;
+  d.bit_alloc_prior = FQB200_PRIOR_STD;
+  d.bit_alloc_round = 1;
+  d.bit_alloc_target = static_cast<float>(num_bits);
+  d.bias_corr = bias_corr ? 1 : 0;
+  d.var_corr = var_corr ? 1 : 0;
+  d.out_hist = hist;
+  return d;
+}
+
+static const char* weights_given_bad_args(int64_t groups, int64_t inner, int32_t num_bits) {
+  if (groups < 0 || inner < 0) return "negative extent%s";
+  if (num_bits < 1 || num_bits > 8) return "num_bits must be in 1..8%s";
+  return nullptr;
+}
+
+size_t fqb200_quantize_weights_given_workspace_bytes(int64_t groups, int64_t inner, int32_t num_bits, int32_t has_bits,
+                                                     int32_t bias_corr, int32_t var_corr) {
+  g_err[0] = 0;
+  const char* bad = weights_given_bad_args(groups, inner, num_bits);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  const fqb200_desc d = weights_given_desc(groups, inner, num_bits, has_bits != 0, bias_corr, var_corr, nullptr);
+  return fqb200_workspace_bytes(&d);
+}
+
+int fqb200_quantize_weights_given(const float* in, float* out, int64_t groups, int64_t inner, const float* delta,
+                                  const float* offset, const float* bits, int32_t num_bits, int32_t bias_corr,
+                                  int32_t var_corr, unsigned long long* hist, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  g_err[0] = 0;
+  const char* bad = weights_given_bad_args(groups, inner, num_bits);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!in || !out || !delta || !offset) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  if (groups == 0 || inner == 0) return FQB200_OK;
+  const fqb200_desc d = weights_given_desc(groups, inner, num_bits, bits != nullptr, bias_corr, var_corr, hist);
+  DeviceInfo* di = nullptr;
+  int rc = get_device(&di);
+  if (rc != FQB200_OK) return rc;
+  FusedPlan fp;
+  rc = plan_fused(&d, aligned16(in) && aligned16(out), 0, *di, &fp);
+  if (rc != FQB200_OK) return rc;
+  rc = check_workspace(workspace, workspace_bytes, fp.workspace, "fqb200_quantize_weights_given_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  carve(static_cast<char*>(workspace), fp.slots, fp.pl.geo.channels, &fp.A);
+  fp.A.in = in;
+  fp.A.out = out;
+  fp.A.g_delta = delta;
+  fp.A.g_offset = offset;
+  fp.A.g_bits = bits;
+  fp.A.given_per_group = 1;
+  void* args[] = {&fp.A};
+  const cudaError_t e = cudaLaunchCooperativeKernel(fp.kernel, dim3(fp.pl.grid), dim3(fp.block), args, fp.smem,
+                                                    static_cast<cudaStream_t>(stream));
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cooperative launch %s: %s", fp.name, cudaGetErrorString(e));
+  return FQB200_OK;
+}
+
+// bit_alloc.allocate's budget: min(floor(target * G), 8 G); -1 when it is negative or not a number
+static int64_t alloc_budget(int64_t groups, double target) {
+  const double b = floor(target * static_cast<double>(groups));
+  if (!(b >= 0.0)) return -1;
+  return b < 8.0 * static_cast<double>(groups) ? static_cast<int64_t>(b) : 8 * groups;
+}
+
+static const char* alloc_bad_args(int64_t groups, double target) {
+  if (groups < 1 || groups > fqb::kAllocMaxGroups) return "groups must be in 1..2^20%s";
+  if (alloc_budget(groups, target) < 0) return "target gives a negative budget%s";
+  return nullptr;
+}
+
+// choice table G x (budget + 1) bytes, then the two best[] rows when they do not fit in shared memory
+static size_t alloc_choice_bytes(int64_t groups, int64_t budget) {
+  return (static_cast<size_t>(groups) * static_cast<size_t>(budget + 1) + 15u) & ~static_cast<size_t>(15u);
+}
+static bool alloc_rows_in_smem(int64_t budget) { return 2u * static_cast<size_t>(budget + 1) * sizeof(double) <= fqb::kAllocMaxSmem; }
+
+size_t fqb200_allocate_widths_workspace_bytes(int64_t groups, double target) {
+  g_err[0] = 0;
+  const char* bad = alloc_bad_args(groups, target);
+  if (bad) return fail(FQB200_ERR_INVALID, bad), 0;
+  const int64_t budget = alloc_budget(groups, target);
+  return alloc_choice_bytes(groups, budget) + (alloc_rows_in_smem(budget) ? 0u : 2u * static_cast<size_t>(budget + 1) * sizeof(double));
+}
+
+int fqb200_allocate_widths(const double* sse, int64_t groups, double target, float* widths_out, int32_t* status,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  g_err[0] = 0;
+  const char* bad = alloc_bad_args(groups, target);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (!sse || !widths_out) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  const int64_t budget = alloc_budget(groups, target);
+  const bool in_smem = alloc_rows_in_smem(budget);
+  const size_t choice = alloc_choice_bytes(groups, budget);
+  int rc = check_workspace(workspace, workspace_bytes, fqb200_allocate_widths_workspace_bytes(groups, target),
+                           "fqb200_allocate_widths_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  const size_t smem = in_smem ? 2u * static_cast<size_t>(budget + 1) * sizeof(double) : 0u;
+  cudaError_t e = setup(fqb::fq_allocate_widths_kernel, fqb::kAllocThreads, smem);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  double* rows = in_smem ? nullptr : reinterpret_cast<double*>(ws + choice);
+  fqb::fq_allocate_widths_kernel<<<1, fqb::kAllocThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+      sse, static_cast<unsigned>(groups), static_cast<unsigned>(budget), ws, rows, widths_out, status);
+  return launched("fq_allocate_widths_kernel");
 }
 
 int fqb200_selftest_division(const float* a, const float* b, float* fast, float* ieee, int64_t n, void* stream) {

@@ -23,7 +23,7 @@ from . import int_quantization
 from . import ops
 from .statistics import refuse_bap_mse
 
-__all__ = ["IntQuantizer", "int_quantizer"]
+__all__ = ["IntQuantizer", "int_quantizer", "WeightMse", "best_candidates", "refuse_clip_weight"]
 
 
 def _laplace_opt_alpha(w):
@@ -63,6 +63,90 @@ def _to_dev(t, device):
     if isinstance(t, torch.Tensor):
         return t.to(device)
     return torch.tensor(t, dtype=torch.float32).to(device)
+
+
+def refuse_clip_weight(clip_weight="mse", per_channel=True, mid_tread=False, bounds=False, qweight="int8", native=True):
+    """Raise where `clip_weight="mse"` cannot run: an unknown value or per-tensor weights (ValueError); the mid-tread
+    (-mtq) bins, explicit min_ / max_ bounds, float weights (qweight f32) or a foreign quantizer (NotImplementedError)."""
+    if clip_weight not in ("no", "mse"):
+        raise ValueError("clip_weight must be 'no' or 'mse', got %r" % (clip_weight,))
+    if clip_weight == "no":
+        return
+    if not per_channel:
+        raise ValueError("clip_weight='mse' picks a clipping value per output channel: it needs per_channel_quant_weights")
+    if mid_tread:
+        raise NotImplementedError("clip_weight='mse' clips the min/max weight quantizer, not the mid-tread (-mtq) bins")
+    if bounds:
+        raise NotImplementedError("clip_weight='mse' measures each row's own range: explicit min_ / max_ bounds are not "
+                                  "supported")
+    if qweight == "f32":
+        raise NotImplementedError("clip_weight='mse' clips quantized weights, and qweight f32 leaves them in float")
+    if not native:
+        raise NotImplementedError("clip_weight='mse' runs on this package's CUDA quantizers only")
+
+
+def best_candidates(err):
+    """(column, error) of the least error per row of ``err`` [G, W, 1 + M] (per channel and width: column 0 the min/max
+    range, then the M clipping values): the first minimum in column order, so min/max wins exact ties and then the
+    earlier multiplier; NaN never wins (statistics.best_columns' rule; a row of NaN keeps min/max)."""
+    pick = torch.where(torch.isnan(err), torch.full_like(err, math.inf), err).argmin(2)
+    return pick, err.gather(2, pick.unsqueeze(2)).squeeze(2)
+
+
+class WeightMse(object):
+    """What `clip_weight="mse"` shares across one model's weight quantizers: the float32 clipping multipliers and their
+    prior ("laplace": alpha = m * b, "gaus": m * std), their device copies, the int32 device flag fqb200_allocate_widths
+    raises on non-finite error tables, and with ``report`` (a CSV path) one row of device sums per quantized weight.
+    Nothing is read back until ``finish``, which reads the flag and the report in one copy."""
+
+    REPORT_COLUMNS = ("id", "rows", "bits", "mse_minmax", "mse_chosen", "kept_minmax", "bits_minmax_alloc",
+                      "mse_minmax_alloc")
+
+    def __init__(self, multipliers, prior, report=None):
+        self.multipliers = np.asarray(multipliers, dtype=np.float32).reshape(-1)
+        self.prior = prior
+        self.report = report
+        self._mult = {}
+        self._status = None
+        self._rows = []   # (id, rows, numel, float64 device [6]: bits, sse min/max, sse chosen, kept, bits / sse of the
+                          # min/max-only allocation)
+
+    def mult(self, dev):
+        m = self._mult.get(dev)
+        if m is None:   # pinned and asynchronous: no host synchronisation inside quantize_model
+            m = self._mult[dev] = torch.from_numpy(self.multipliers).pin_memory().to(dev, non_blocking=True)
+        return m
+
+    def status(self, dev):
+        if self._status is None:
+            self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        return self._status
+
+    def add(self, id, rows, numel, sums):
+        if self.report is not None:
+            self._rows.append((id, rows, numel, sums))
+
+    def finish(self):
+        """Read the flag and the report sums back (one copy), write the report, and raise ValueError when an allocation
+        met a non-finite error."""
+        if self._status is None and not self._rows:
+            return
+        parts = ([self._status.double()] if self._status is not None else []) + [r[3] for r in self._rows]
+        host = torch.cat([p.reshape(-1).to(parts[0].device) for p in parts]).cpu().numpy()
+        bad = self._status is not None and host[0] != 0
+        sums = host[1 if self._status is not None else 0:].reshape(-1, 6)
+        rows, self._rows, self._status = self._rows, [], None
+        if self.report is not None and rows:
+            import csv
+            with open(self.report, "w", newline="") as f:
+                w = csv.writer(f)
+                w.writerow(self.REPORT_COLUMNS)
+                for (id, r, n, _), s in zip(rows, sums):
+                    w.writerow([id, r, int(s[0]), repr(float(s[1] / n)), repr(float(s[2] / n)), int(s[3]),
+                                "" if np.isnan(s[4]) else int(s[4]), "" if np.isnan(s[5]) else repr(float(s[5] / n))])
+        if bad:
+            raise ValueError("clip_weight='mse': a weight's error table holds NaN or Inf, so its width allocation is not "
+                             "defined (bit_alloc.allocate refuses such tables)")
 
 
 # A call site's `-sm use` parameters: per channel, [C] delta / offset and the widths (or None) of the torch leaf; per
@@ -112,6 +196,10 @@ class IntQuantizer(object):
         self.mse_curves = None
         # `-bap mse`: the statistics.BitMseStatistics that reads the collected per-channel error tables (set by the manager)
         self.bit_tables = None
+        # `clip_weight="mse"` (set by the manager on its weight quantizers): per output channel the measured best of the
+        # min/max range and the clipping candidates of ``weight_mse`` (a WeightMse)
+        self.clip_weight = "no"
+        self.weight_mse = None
         self._stat_cache = {}  # offline-statistics parameters are constants of a layer: solved once, kept on the device
         self.force_positive = False
         self.half_range = False
@@ -123,6 +211,7 @@ class IntQuantizer(object):
         # (columns _lib.STAT_COLUMNS) in ``last_stats`` - what the parity tests compare with the reference's values
         self.export_stats = False
         self.last_stats = None
+        self.last_weight_mse = None   # ... and of the most recent `clip_weight="mse"` weight (see _clip_mse_weights)
         # per-call inputs of ``__call__``'s extensions (reset when the call returns)
         self._relu_follows, self._bca, self._residual, self._defer, self._pool, self._into = False, None, None, False, None, None
 
@@ -692,6 +781,7 @@ class IntQuantizer(object):
         rows = tensor.shape[0]
         layout = (1, rows, tensor.numel() // rows)
         if min_ is not None or max_ is not None:
+            refuse_clip_weight(self.clip_weight, bounds=True)
             t = tensor.reshape(rows, -1)
             mn = _to_dev(min_, tensor.device) if min_ is not None else t.min(-1)[0]
             mx = _to_dev(max_, tensor.device) if max_ is not None else t.max(-1)[0]
@@ -703,6 +793,8 @@ class IntQuantizer(object):
                 bits = self.get_bits_alloc_fixed_target(t.std(-1), self.bit_alloc_target_weight, self.bit_alloc_round)
             return ops.quantize1(tensor, mx - mn, mn, self.num_bits, bits=bits, layout=layout)
         bc, vc = weight_correction if weight_correction is not None else (False, False)
+        if self.clip_weight == "mse":
+            return self._clip_mse_weights(tensor, id, layout, bc, vc)
         if self.bit_alloc_weight and self.num_bits <= 4 and self.bit_alloc_prior == "mse":
             return self._mse_weights(tensor, id, layout, bc, vc)
         hist = self._hist(tensor)
@@ -737,6 +829,60 @@ class IntQuantizer(object):
             from .manager import QuantizationManagerInference
             res = QuantizationManagerInference._weight_correction_torch(tensor.contiguous(), res.contiguous(), bias_corr,
                                                                         var_corr)
+        return res
+
+    def _clip_mse_weights(self, tensor, id, layout, bias_corr, var_corr, max_ctas=0):
+        """`clip_weight="mse"`: per output channel the candidate with the least measured squared error among the min/max
+        range (first: it wins exact ties) and the clipping values of ``weight_mse`` (in their order; NaN never wins), at
+        the channel's width - ``num_bits``; with `-baw`, the width the default launch's bit allocation gives it, or under
+        `-bap mse` the widths fqb200_allocate_widths picks from the per-width best errors.  A statistics-only launch, the
+        candidates' errors and parameters (ops.clip_mse_grid, ops.clip_mse with prior "minmax"), the selection as device
+        tensor ops, and one ops.quantize_weights_given launch with the call's corrections and `-me` histogram, which runs
+        the chosen parameters exactly as they were measured.  A channels-last weight is read in NCHW order throughout and
+        the result comes back in it.  Nothing is read back to the host."""
+        wm = self.weight_mse
+        dev = tensor.device
+        g = layout[1]
+        alloc = bool(self.bit_alloc_weight and self.num_bits <= 4)
+        table = ops.fused(tensor, layout, num_bits=self.num_bits, bit_alloc=self.bit_alloc_weight,
+                          bit_alloc_prior=L.PRIOR_STD, bit_alloc_round=self.bit_alloc_round,
+                          bit_alloc_target=self.bit_alloc_target_weight, stats_only=True)
+        widths = list(range(9)) if alloc else [self.num_bits]
+        nw = len(widths)
+        mult = wm.mult(dev)
+        m = mult.numel()
+        grid, gp = ops.clip_mse_grid(tensor, table, layout, False, self.num_bits, False, mult, widths, prior=wm.prior,
+                                     want_params=True, max_ctas=max_ctas)
+        mm, mp = ops.clip_mse(tensor, table, layout, False, self.num_bits, False, torch.zeros(nw, device=dev),
+                              prior="minmax", widths=widths, want_params=True, max_ctas=max_ctas)
+        err = torch.cat([mm[:, 1:].reshape(g, nw, 1), grid[:, 1:].reshape(g, nw, m)], 2)
+        par = torch.cat([mp.reshape(g, nw, 1, 6), gp.reshape(g, nw, m, 6)], 2)
+        pick, best = best_candidates(err)
+        if not alloc:
+            wi = torch.zeros(g, dtype=torch.int64, device=dev)
+        elif self.bit_alloc_prior == "mse":
+            wi = ops.allocate_widths(best, self.bit_alloc_target_weight, wm.status(dev)).long()
+        else:
+            wi = table[:, 7].long()
+        k = pick.gather(1, wi.unsqueeze(1)).squeeze(1)
+        p = par[torch.arange(g, device=dev), wi, k]
+        bits = p[:, 2].contiguous() if alloc else None
+        hist = self._hist(tensor)
+        res = ops.quantize_weights_given(tensor, p[:, 0].contiguous(), p[:, 1].contiguous(), self.num_bits, bits=bits,
+                                         bias_corr=bias_corr, var_corr=var_corr, hist=hist)
+        self._log_entropy(hist, id, "avg.entropy.weight", tensor.numel())
+        if self.export_stats:   # per channel: the chosen candidate's error, min/max's error at its width, the width
+            self.last_weight_mse = (best.gather(1, wi.unsqueeze(1)).squeeze(1), mm[:, 1:].gather(1, wi.unsqueeze(1)).squeeze(1),
+                                    p[:, 2])
+        if wm.report is not None:
+            nan = torch.full((), math.nan, dtype=torch.float64, device=dev)
+            ref_bits, ref_sse = nan, nan
+            if alloc and self.bit_alloc_prior == "mse":   # today's min/max-only allocation for the same budget
+                wmm = ops.allocate_widths(mm[:, 1:], self.bit_alloc_target_weight, wm.status(dev)).long()
+                ref_bits, ref_sse = wmm.sum().double(), mm[:, 1:].gather(1, wmm.unsqueeze(1)).sum()
+            wm.add(id, g, tensor.numel(), torch.stack([
+                p[:, 2].double().sum(), mm[:, 1:].gather(1, wi.unsqueeze(1)).sum(), best.gather(1, wi.unsqueeze(1)).sum(),
+                (k == 0).sum().double(), ref_bits, ref_sse]))
         return res
 
     # mid-tread "bin allocation" quantizer, int_quantizer.py:147-225

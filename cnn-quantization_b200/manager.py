@@ -45,7 +45,11 @@ def make_args(**over):
     together) and
     ``measure_stats_kind`` (what `-ms` measures: "distance", the reference's default squared norms; "angle", the
     pairwise sample angles of its angle_stats module, which the reference selects by editing an import; or "noise", the
-    per-sample quantization error statistics of its measure_statistics module, which the reference cannot run)."""
+    per-sample quantization error statistics of its measure_statistics module, which the reference cannot run),
+    ``clip_weight`` ("no" or "mse": quantize each output channel of a per-channel weight at the least measured squared
+    error among its min/max range and the ``mse_multipliers`` clipping values under ``mse_prior``, at the widths `-baw`
+    gives it or, with `-bap mse`, at the widths that minimise the sum of those least errors) and ``weight_mse_report`` (a
+    CSV path: one row per weight quantized under clip_weight "mse", written after quantize_model)."""
     d = dict(arch="resnet18", qtype=None, qweight="int8", q_off=False, clipping="no", stats_mode="no", stats_kind="mean",
              stats_folder=None, stats_batch_avg=False, kld_threshold=False, measure_stats=False,
              per_channel_quant_weights=False, per_channel_quant_act=False, bit_alloc_act=False, bit_alloc_weight=False,
@@ -53,7 +57,7 @@ def make_args(**over):
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
              mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
              collect_err=False, measure_stats_kind="distance", collect_mse=False, mse_multipliers=None, mse_prior="laplace",
-             collect_bits=False)
+             collect_bits=False, clip_weight="no", weight_mse_report=None)
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -392,6 +396,19 @@ class QuantizationManagerInference(object):
         # the pooled quarter - so they are switched off; each is bit-identical to its unfused form.
         # The noise kind also measures the tensor the quantizer was handed, so activations are quantized out of place and
         # that tensor survives the launch; the convolution bias stays fused and is passed to the measurement.
+        # `clip_weight="mse"`: measured clipping of the per-channel weights, shared by the weight quantizers
+        from .int_quantizer import WeightMse, refuse_clip_weight
+        clip_weight = getattr(args, "clip_weight", "no")
+        refuse_clip_weight(clip_weight, args.per_channel_quant_weights, args.mid_thread_quant, qweight=args.qweight,
+                           native=self._native)
+        report = getattr(args, "weight_mse_report", None)
+        if report is not None and clip_weight != "mse":
+            raise ValueError("weight_mse_report reports the weights quantized under clip_weight='mse'")
+        self.weight_mse = None
+        if clip_weight == "mse":
+            from .statistics import _mse_multipliers
+            prior = getattr(args, "mse_prior", "laplace")
+            self.weight_mse = WeightMse(_mse_multipliers(getattr(args, "mse_multipliers", None), prior), prior, report)
         self.measure_stats = None
         kind = getattr(args, "measure_stats_kind", "distance")
         if kind not in ("distance", "angle", "noise"):
@@ -499,6 +516,9 @@ class QuantizationManagerInference(object):
         if self.quantize:
             self.__fill_quantizers__(args.qtype, qparams, args.arch, args.qweight)
             self.quantizer_default = self._load("int8", qparams)
+            if self.weight_mse is not None:
+                for tag in ("weight", "weight_classifier"):
+                    self.quantizers[tag].clip_weight, self.quantizers[tag].weight_mse = "mse", self.weight_mse
             if self.stats_mode == "use":
                 # which statistics each tag reads (IntQuantizer.__init__ :88 + the overrides of __fill_quantizers__)
                 per_tensor = lambda: self._sm_tensor
@@ -908,6 +928,8 @@ class QuantizationManagerInference(object):
             if any(corr) and not extra:
                 weight_q = self._weight_correction_torch(m.weight.data, weight_q, *corr)
             m.weight.data = weight_q
+        if self.weight_mse is not None:
+            self.weight_mse.finish()   # the one read-back of clip_weight="mse": its report and its non-finite flag
 
     @staticmethod
     def _weight_correction_torch(w, w_q, bias_corr, var_corr):

@@ -26,7 +26,8 @@ def profile_collect():
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
     (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'N' the quantization-noise measurement
     (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error), 'R' the clipping-MSE curves (ops.clip_mse)
-    and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing."""
+    and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing; 'W' the given-parameter
+    weight launch with its corrections (ops.quantize_weights_given) and 'L' the width allocation (ops.allocate_widths)."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -699,6 +700,62 @@ def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multiplie
                 int(bool(positive)), 0, int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), m,
                 widths.ctypes.data, widths.size, out.data_ptr(), _ptr(params), ws.data_ptr(), ws.numel(), int(max_ctas))
     return (out, params) if want_params else out
+
+
+def quantize_weights_given(w, delta, offset, num_bits, bits=None, bias_corr=False, var_corr=False, hist=None):
+    """C ABI fqb200_quantize_weights_given: per-output-channel quantization of a weight ([O, ...], read in NCHW order,
+    copied when not contiguous) with given float32 [O] device ``delta`` / ``offset`` / ``bits`` (None: ``num_bits``) and the
+    `-vcw` / `-bcw` corrections of the RANGE_MINMAX weight launch, in one launch.  ``hist``: 256 int64 counters of the
+    integer grid (`-me`), accumulated.  Returns the contiguous result.  Recorded in the launch profile under mode 'W'."""
+    _require_cuda_f32(w, "weight")
+    lib = L.load()
+    w = w.contiguous()
+    dev = w.device
+    groups = w.shape[0]
+    inner = w.numel() // groups if groups else 0
+    vecs = []
+    for name, v in (("delta", delta), ("offset", offset), ("bits", bits)):
+        if v is not None:
+            _require_cuda_f32(v, name)
+            v = v.contiguous()
+            if v.numel() != groups:
+                raise ValueError("%s must have %d elements" % (name, groups))
+        vecs.append(v)
+    if hist is not None and (hist.dtype != torch.int64 or not hist.is_cuda or not hist.is_contiguous() or hist.numel() != 256):
+        raise ValueError("hist must be a contiguous CUDA int64 tensor of 256 counters")
+    out = torch.empty_like(w)
+    if w.numel() == 0:
+        return out
+    with torch.cuda.device(dev):
+        need = lib.fqb200_quantize_weights_given_workspace_bytes(groups, inner, int(num_bits), int(bits is not None),
+                                                                 int(bool(bias_corr)), int(bool(var_corr)))
+        if need == 0:
+            L.check(L.ERR_INVALID)
+        ws = _workspace(dev, _stream_handle(dev), need)
+    _launch(dev, _Timed("W", w.numel(), 16 if var_corr else 12, "%dx%d" % (groups, inner)),
+            lib.fqb200_quantize_weights_given, w.data_ptr(), out.data_ptr(), groups, inner, vecs[0].data_ptr(),
+            vecs[1].data_ptr(), _ptr(vecs[2]), int(num_bits), int(bool(bias_corr)), int(bool(var_corr)), _ptr(hist),
+            ws.data_ptr(), ws.numel())
+    return out
+
+
+def allocate_widths(sse, target, status=None):
+    """C ABI fqb200_allocate_widths: float32 [G] device widths in 0..8 that minimise the sum of the float64 [G, 9] device
+    table ``sse`` for the budget of ``target`` bits per channel - bit_alloc.allocate's result, bit for bit, without a host
+    round trip.  ``status``: an int32 device tensor set to 1 when ``sse`` holds a non-finite value (never cleared)."""
+    if not (isinstance(sse, torch.Tensor) and sse.is_cuda and sse.dtype == torch.float64 and sse.dim() == 2
+            and sse.shape[1] == 9):
+        raise ValueError("allocate_widths needs a float64 [G, 9] CUDA table")
+    if status is not None and (status.dtype != torch.int32 or status.device != sse.device):
+        raise ValueError("status must be an int32 tensor on the table's device")
+    lib = L.load()
+    sse = sse.contiguous()
+    groups = sse.shape[0]
+    ws = _own_workspace(sse.device, lib.fqb200_allocate_widths_workspace_bytes(groups, float(target)))
+    out = torch.empty(groups, dtype=torch.float32, device=sse.device)
+    _launch(sse.device, _Timed("L", groups, 72), lib.fqb200_allocate_widths, sse.data_ptr(), groups, float(target),
+            out.data_ptr(), _ptr(status), ws.data_ptr(), ws.numel())
+    return out
 
 
 KMeans1d =collections.namedtuple("KMeans1d", "labels centres inertia n_iter init_ids out out_bcorr")

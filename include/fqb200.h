@@ -461,6 +461,44 @@ int fqb200_kmeans1d(const float* in, int64_t n, int32_t num_bits, int64_t first_
  * two in 2 .. 256 or n < k). */
 size_t fqb200_kmeans1d_workspace_bytes(int64_t n, int32_t k);
 
+/*
+ * Per-channel weight quantization with given parameters and the weight corrections (`clip_weight="mse"`): the rows
+ * [groups][inner] of a contiguous NCHW-ordered weight ([O][I*k*k]) through the torch leaf with the caller's per-row device
+ * vectors delta, offset and (optional, NULL = num_bits everywhere) bits, then the correction phases of the FQB200_RANGE_MINMAX
+ * weight launch of fqb200_fused: var_corr (`-vcw`) first, then bias_corr (`-bcw`), from the float64 row means and stds of
+ * `in`.  hist (optional): 256 int64 counters of the integer grid, accumulated (`-me`).  It runs that launch's plan
+ * (bits given = its bit allocation), with the solve replaced by the given parameters, so given the delta, offset and bits
+ * columns (5, 6, 7) a RANGE_MINMAX weight launch reports in its statistics table, `out` has that launch's bits, with or
+ * without corrections, bit allocation and histogram.  One cooperative launch on `stream`, no host synchronisation.  The
+ * workspace (fqb200_quantize_weights_given_workspace_bytes, the same for any `bits` pointer of the same nullness) is the
+ * shared one of fqb200_fused (fqb200_workspace_init).  FQB200_ERR_INVALID, before any CUDA call: negative extents,
+ * num_bits outside 1..8, a null in, out, delta or offset.
+ */
+int fqb200_quantize_weights_given(const float* in, float* out, int64_t groups, int64_t inner, const float* delta,
+                                  const float* offset, const float* bits, int32_t num_bits, int32_t bias_corr,
+                                  int32_t var_corr, unsigned long long* hist, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+/* Workspace of fqb200_quantize_weights_given in bytes (0 and fqb200_last_error() on arguments it does not take). */
+size_t fqb200_quantize_weights_given_workspace_bytes(int64_t groups, int64_t inner, int32_t num_bits, int32_t has_bits,
+                                                     int32_t bias_corr, int32_t var_corr);
+/*
+ * Exact per-channel bit allocation on the device, the result of bit_alloc.allocate bit for bit: the float32 widths_out[G]
+ * in 0..8 minimising sum_g sse[g][w_g] (sse: device float64 [G][9], the error of channel g at width w) subject to
+ * sum_g w_g <= min(floor(target * G), 8 G); among minimisers the lexicographically smallest width vector.  The same
+ * dynamic programme from the last channel to the first, with the same float64 sums in the same order and the strict `<`
+ * per width in increasing width order, in one CTA (fq_alloc.cuh).  The host function refuses non-finite errors; here NaN
+ * never wins a comparison and any non-finite entry sets *status (optional, device int32) to 1 - it is never cleared, so
+ * one flag can collect a whole model.  One launch on `stream`, no host synchronisation.  Workspace
+ * (fqb200_allocate_widths_workspace_bytes, private to the call, no initialisation): the uint8 choice table G x (budget +
+ * 1), plus the two float64 best[] rows when they exceed 227 KB of shared memory.  FQB200_ERR_INVALID, before any CUDA call:
+ * G outside 1..2^20, a negative or NaN budget, a null sse or widths_out; FQB200_ERR_WORKSPACE: a workspace that is missing,
+ * too small or misaligned.
+ */
+int fqb200_allocate_widths(const double* sse, int64_t groups, double target, float* widths_out, int32_t* status,
+                           void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace of fqb200_allocate_widths in bytes (0 and fqb200_last_error() on arguments it does not take). */
+size_t fqb200_allocate_widths_workspace_bytes(int64_t groups, double target);
+
 #ifdef __cplusplus
 }
 #endif
