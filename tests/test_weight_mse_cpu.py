@@ -1,6 +1,7 @@
 """Measured clipping of weights (`clip_weight="mse"`) without a GPU: the two new C entry points in the header and the
 export table and their argument checks, the manager's flags and refusals, the defaults that leave the reference's
-parameter dict alone, and a float64 restatement of the per-channel candidate selection."""
+parameter dict alone, a float64 restatement of the per-channel candidate selection, and the whole-chain restatement
+(tests/golden/weight_mse_oracle.py) on hand-sized rows with hand-computed answers."""
 import ctypes
 import json
 import math
@@ -200,3 +201,73 @@ def test_selection_rule_on_hand_made_tables():
         want_pick, want_best = _select_f64(e)
         assert np.array_equal(pick.numpy(), want_pick)
         assert np.array_equal(best.numpy(), want_best, equal_nan=True)
+
+
+# ---- the float64 restatement (tests/golden/weight_mse_oracle.py) on hand-sized rows ---------------------------------------------
+def test_restatement_constant_and_zero_rows():
+    """A constant row has b = std = 0: every clipping value gives offset = the value and delta = 0, the min/max range's
+    parameters, so every candidate makes the same error and min/max is kept; an all-zero row quantizes to 0 exactly."""
+    import weight_mse_oracle as W
+    w = np.array([[0.5] * 4, [0.0] * 4], dtype=np.float32)
+    st = W.row_stats(w)
+    assert st.tolist() == [[0.5, 0.5, 0.5, 0.0, 0.0], [0.0] * 5]
+    for prior in ("laplace", "gaus"):
+        r = W.restate(w, W.table_from_stats(st), [0.5, 1.0, 8.0], prior, 4)
+        assert r["delta"].tolist() == [[0.0] * 4] * 2 and r["offset"].tolist() == [[0.5] * 4, [0.0] * 4]
+        assert (r["err"] == r["err"][..., :1]).all() and r["err"][1].tolist() == [[0.0] * 4]
+        assert r["pick"].tolist() == [[0], [0]] and r["report"]["kept_minmax"] == 2
+        assert r["y"][1].tolist() == [0.0] * 4
+
+
+def test_restatement_exact_tie_between_two_multipliers():
+    """Row (0, -3, 3): mean 0, b 2.  At 1 bit (qmax 1, round half to even):
+      min/max   offset -3, delta 6, scale 6, zero point rint(0.5) = 0: q = 0, 0, 0    -> error 0 + 9 + 9 = 18
+      m = 0.5   alpha 1: offset -1, delta 2, scale 2, zero point 0:  q = 0, 0, 1 (y 2) -> error 0 + 9 + 1 = 10
+      m = 1.0   alpha 2: offset -2, delta 4, scale 4, zero point 0:  q = 0, 0, 1 (y 4) -> error 0 + 9 + 1 = 10
+      m = 1.5   alpha 3: offset -3, delta 6: the min/max parameters                   -> 18
+    so the earlier of the two tied multipliers wins.  At 2 bits min/max (scale 2, zero point 2: y = 0, -4, 2) and m = 1.5
+    both make error 2, the least, and min/max is kept."""
+    import weight_mse_oracle as W
+    w = np.array([[0.0, -3.0, 3.0]], dtype=np.float32)
+    t = W.table_from_stats(W.row_stats(w))
+    assert t[0, :4].tolist() == [-3.0, 3.0, 0.0, 2.0]
+    r = W.restate(w, t, [0.5, 1.0, 1.5], "laplace", 1)
+    assert r["delta"].tolist() == [[6.0, 2.0, 4.0, 6.0]] and r["offset"].tolist() == [[-3.0, -1.0, -2.0, -3.0]]
+    assert r["err"].tolist() == [[[18.0, 10.0, 10.0, 18.0]]]
+    assert r["pick"].tolist() == [[1]] and r["y0"].tolist() == [[0.0, 0.0, 2.0]]
+    assert r["report"]["kept_minmax"] == 0 and r["report"]["mse_chosen"] == 10.0 / 3 and r["report"]["mse_minmax"] == 6.0
+    r = W.restate(w, t, [0.5, 1.0, 1.5], "laplace", 2)
+    assert r["err"][0, 0, 0] == r["err"][0, 0, 3] == 2.0 and r["pick"].tolist() == [[0]]
+    assert r["y0"].tolist() == [[0.0, -4.0, 2.0]] and r["report"]["kept_minmax"] == 1
+
+
+def test_restatement_nan_candidate_never_wins():
+    """A one-element row has no unbiased std (0 / 0): with the gaus prior every clipping value is NaN, its candidates' errors
+    are NaN, and the min/max range (delta 0: the 1e-8 scale floor) is kept.  With the Laplace prior b = 0 and every
+    candidate is the min/max range."""
+    import weight_mse_oracle as W
+    w = np.array([[0.75], [-2.0]], dtype=np.float32)
+    st = W.row_stats(w)
+    assert np.isnan(st[:, 4]).all() and (st[:, 3] == 0).all()
+    r = W.restate(w, W.table_from_stats(st), [1.0, 2.0], "gaus", 4)
+    assert np.isnan(r["err"][:, :, 1:]).all() and np.isfinite(r["err"][:, :, 0]).all()
+    assert r["pick"].tolist() == [[0], [0]] and r["chosen"][0].tolist() == [0.0, 0.0]
+    assert r["chosen"][1].tolist() == [0.75, -2.0]
+    assert np.abs(r["y0"] - w).max() <= 1e-8
+    r = W.restate(w, W.table_from_stats(st), [1.0, 2.0], "laplace", 4)
+    assert (r["err"] == r["err"][..., :1]).all() and r["pick"].tolist() == [[0], [0]]
+
+
+def test_restatement_allocates_zero_bits_to_a_zero_row():
+    """Under -bap mse the zero row's error is 0 at every width, so bit_alloc.allocate gives it 0 bits (ties take the smaller
+    width) and the whole budget of 2 x 4 bits goes to the other row, whose error falls with every bit."""
+    import weight_mse_oracle as W
+    from cnn_quantization_b200.bit_alloc import allocate
+    w = np.array([[0.0, 0.0, 0.0], [0.0, -3.0, 3.0]], dtype=np.float32)
+    r = W.restate(w, W.table_from_stats(W.row_stats(w)), [0.5, 1.0, 1.5], "laplace", 4, baw=True, bap_mse=True)
+    assert r["widths"] == list(range(9)) and (r["err"][0] == 0).all()
+    assert (np.diff(r["best"][1]) < 0).all()
+    assert r["wi"].tolist() == [0, 8] and allocate(r["best"], 4).tolist() == [0, 8]
+    assert r["chosen"][2].tolist() == [0.0, 8.0] and r["report"]["bits"] == 8
+    assert r["y0"][0].tolist() == [0.0] * 3
+    assert r["report"]["bits_minmax_alloc"] == 8 and r["report"]["mse_minmax_alloc"] == r["err"][1, 8, 0] / 6
