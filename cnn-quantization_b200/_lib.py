@@ -75,6 +75,8 @@ PROTOTYPES = {
                                _i32, _vp]),
     "fqb200_clip_mse_widths": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _vp,
                                       _vp, _sz, _i32, _vp]),
+    "fqb200_clip_mse_select": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _vp,
+                                      _vp, _vp, _vp, _vp, _sz, _i32, _vp]),
     "fqb200_clip_mse_workspace_bytes": (_sz, [_i64, _i64, _i64, _i32, _i32]),
     "fqb200_clip_mse_grid": (_i32, [_vp, _i64, _i64, _i64, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _i32, _vp,
                                     _vp, _vp, _sz, _i32, _vp]),

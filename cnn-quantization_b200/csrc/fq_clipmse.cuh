@@ -28,7 +28,9 @@
 //                              warp / CTA tree adds the tile into the unit's shared-memory sums.  Each unit writes its own
 //                              workspace slot; sum x^2 comes from the units of width 0 only.
 //   fq_clipmse_finish_kernel   one CTA per group: adds the group's unit partials in chunk order, writes out[g] and,
-//                              optionally, the candidates' parameters.
+//                              optionally, the candidates' parameters.  A select launch (fqb200_clip_mse_select, `-c mse`
+//                              on the fly) then picks the group's column in statistics.best_columns' order (cm_before)
+//                              with one warp over the final sums, and writes that candidate's parameters.
 //
 // No atomics touch the values: the result has the same bits on every run and for every grid size.  NaN propagates.
 namespace fqb {
@@ -60,6 +62,9 @@ struct ClipMseArgs {
   double* partial;                     // [groups][units_per_group][nw * K + 1]
   double* out;                         // [groups][nw * K + 1]
   float* params;                       // optional [groups][nw * K][kCeParams]
+  int* choice;                         // select launch: [groups] chosen column (nullptr: no selection)
+  float* given;                        // select launch: [3][groups] chosen delta, offset, bits
+  float* table;                        // select launch, optional: [groups][FQB200_STATS_STRIDE] parameter table
 };
 
 // candidate k (of width index wi in a grid launch) of group g: alpha = mult[k] * (b or std) - solve_range's k-std rule
@@ -267,6 +272,53 @@ __global__ void __launch_bounds__(kCmThreads, 2) fq_clipmse_partial_kernel(const
   }
 }
 
+// one candidate in the selection: its error (NaN read as +inf, so it never wins), multiplier and column (-1: none)
+struct CmPick {
+  double e;
+  float m;
+  int k;
+};
+// true when a goes before b in statistics.best_columns' order: the smaller error, then the smaller multiplier (NaN
+// last, as np.argsort puts it), then the earlier column.  A total order, so the warp's tree gives the same pick as a scan.
+__device__ __forceinline__ bool cm_before(const CmPick& a, const CmPick& b) {
+  if (a.k < 0 || b.k < 0) return b.k < 0 && a.k >= 0;
+  if (a.e != b.e) return a.e < b.e;
+  const bool an = isnan(a.m), bn = isnan(b.m);
+  if (an != bn) return bn;
+  if (!an && a.m != b.m) return a.m < b.m;
+  return a.k < b.k;
+}
+
+// the select launch's tail, warp 0 of group g's finish CTA once out[g] is final: the chosen column and its candidate's
+// (delta, offset, bits) and leaf, exactly as cm_candidate gives them to out_params
+__device__ __forceinline__ void cm_select(const ClipMseArgs& A, unsigned long long g) {
+  const double* e = A.out + g * (A.K + 1) + 1;
+  CmPick p{0.0, 0.f, -1};
+  for (int k = threadIdx.x; k < A.K; k += 32) {
+    const double ek = e[k];
+    const CmPick c{isnan(ek) ? static_cast<double>(INFINITY) : ek, __ldg(A.mult + k), k};
+    if (cm_before(c, p)) p = c;
+  }
+  for (int o = 16; o; o >>= 1) {
+    const CmPick c{__shfl_xor_sync(0xffffffffu, p.e, o), __shfl_xor_sync(0xffffffffu, p.m, o),
+                   __shfl_xor_sync(0xffffffffu, p.k, o)};
+    if (cm_before(c, p)) p = c;
+  }
+  if (threadIdx.x != 0) return;
+  float d, o, b;
+  const LeafParam q = cm_candidate(A, g, p.k, 0, d, o, b);
+  A.choice[g] = p.k;
+  A.given[g] = d;
+  A.given[A.groups + g] = o;
+  A.given[2 * A.groups + g] = b;
+  if (A.table) {
+    const float* t = A.stats + g * FQB200_STATS_STRIDE;
+    float* dst = A.table + g * FQB200_STATS_STRIDE;
+    for (int c = 0; c < 5; ++c) dst[c] = t[c];
+    dst[5] = d; dst[6] = o; dst[7] = b; dst[8] = q.a; dst[9] = q.b; dst[10] = q.c; dst[11] = static_cast<float>(q.flags);
+  }
+}
+
 __global__ void __launch_bounds__(kCmThreads) fq_clipmse_finish_kernel(const __grid_constant__ ClipMseArgs A) {
   const unsigned long long g = blockIdx.x;
   const int n = A.nw * A.K, W = n + 1;
@@ -284,6 +336,10 @@ __global__ void __launch_bounds__(kCmThreads) fq_clipmse_finish_kernel(const __g
       float* dst = A.params + (g * n + j) * kCeParams;
       dst[0] = d; dst[1] = o; dst[2] = b; dst[3] = q.a; dst[4] = q.b; dst[5] = q.c;
     }
+  }
+  if (A.choice) {
+    __syncthreads();   // the group's sums in out[g] are final and visible to the CTA
+    if (threadIdx.x < 32) cm_select(A, g);
   }
 }
 

@@ -2669,13 +2669,14 @@ int fqb200_clip_mse(const float* in, int64_t outer, int64_t groups, int64_t inne
                                 stream);
 }
 
-// the launch of fqb200_clip_mse_widths and fqb200_clip_mse_grid after their argument checks: K candidates per unit, nw
-// units per (group, chunk) - nw widths[i] of a grid launch, else 1 (widths, when given, one per candidate)
+// the launch of fqb200_clip_mse_widths, fqb200_clip_mse_select and fqb200_clip_mse_grid after their argument checks: K
+// candidates per unit, nw units per (group, chunk) - nw widths[i] of a grid launch, else 1 (widths, when given, one per
+// candidate); with `choice`, the finish kernel also selects each group's candidate
 static int clipmse_launch(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
                           int32_t prior, const float* multipliers, int32_t K, const int32_t* widths, int32_t nw, bool grid,
-                          double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
-                          void* stream, const char* sizer) {
+                          double* out, float* out_params, int32_t* choice, float* given, float* out_table,
+                          void* workspace, size_t workspace_bytes, int32_t max_ctas, void* stream, const char* sizer) {
   int rc = check_workspace(workspace, workspace_bytes, clipmse_workspace(outer, groups, inner, channels_last, nw * K), sizer);
   if (rc != FQB200_OK) return rc;
   DeviceInfo* di = nullptr;
@@ -2708,6 +2709,9 @@ static int clipmse_launch(const float* in, int64_t outer, int64_t groups, int64_
   A.partial = static_cast<double*>(workspace);
   A.out = out;
   A.params = out_params;
+  A.choice = choice;
+  A.given = given;
+  A.table = out_table;
   const int grid_ctas = grid_for(A.units, di->sms * 2ull, max_ctas);
   if (channels_last) {
     fqb::fq_clipmse_partial_kernel<2><<<grid_ctas, fqb::kCmThreads, fqb::cm_smem_bytes(A.K, fqb::kCmSlab), st>>>(A);
@@ -2720,12 +2724,12 @@ static int clipmse_launch(const float* in, int64_t outer, int64_t groups, int64_
   return launched("clipping-MSE kernels");
 }
 
-int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+// fqb200_clip_mse_widths' argument checks, then its launch (with a selection when `choice` is given)
+static int clipmse_checked(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                            const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
                            int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
-                           double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
-                           void* stream) {
-  g_err[0] = 0;
+                           double* out, float* out_params, int32_t* choice, float* given, float* out_table, void* workspace,
+                           size_t workspace_bytes, int32_t max_ctas, void* stream) {
   const char* bad = clipmse_bad_args(outer, groups, inner, channels_last, num_multipliers);
   if (bad) return fail(FQB200_ERR_INVALID, bad);
   if (!in || !stats || !multipliers || !out) return fail(FQB200_ERR_INVALID, "null pointer%s");
@@ -2742,8 +2746,31 @@ int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64
   }
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
   return clipmse_launch(in, outer, groups, inner, channels_last, stats, num_bits, positive, bit_alloc, solve_f64, prior,
-                        multipliers, num_multipliers, widths, 1, false, out, out_params, workspace, workspace_bytes, max_ctas,
-                        stream, "fqb200_clip_mse_workspace_bytes");
+                        multipliers, num_multipliers, widths, 1, false, out, out_params, choice, given, out_table, workspace,
+                        workspace_bytes, max_ctas, stream, "fqb200_clip_mse_workspace_bytes");
+}
+
+int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                           int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
+                           double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
+                           void* stream) {
+  g_err[0] = 0;
+  return clipmse_checked(in, outer, groups, inner, channels_last, stats, num_bits, positive, bit_alloc, solve_f64, prior,
+                         multipliers, widths, num_multipliers, out, out_params, nullptr, nullptr, nullptr, workspace,
+                         workspace_bytes, max_ctas, stream);
+}
+
+int fqb200_clip_mse_select(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                           int32_t prior, const float* multipliers, int32_t num_multipliers, double* out, float* out_params,
+                           int32_t* choice, float* given, float* out_table, void* workspace, size_t workspace_bytes,
+                           int32_t max_ctas, void* stream) {
+  g_err[0] = 0;
+  if (!choice || !given) return fail(FQB200_ERR_INVALID, "null pointer%s");
+  return clipmse_checked(in, outer, groups, inner, channels_last, stats, num_bits, positive, bit_alloc, solve_f64, prior,
+                         multipliers, nullptr, num_multipliers, out, out_params, choice, given, out_table, workspace,
+                         workspace_bytes, max_ctas, stream);
 }
 
 // the layouts, multiplier and width counts fqb200_clip_mse_grid takes (argument errors as a message, nullptr when fine)
@@ -2784,8 +2811,8 @@ int fqb200_clip_mse_grid(const float* in, int64_t outer, int64_t groups, int64_t
   }
   if (max_ctas < 0) return fail(FQB200_ERR_INVALID, "max_ctas must be >= 0%s");
   return clipmse_launch(in, outer, groups, inner, channels_last, stats, num_bits, positive, 0, solve_f64, prior,
-                        multipliers, num_multipliers, widths, num_widths, true, out, out_params, workspace, workspace_bytes,
-                        max_ctas, stream, "fqb200_clip_mse_grid_workspace_bytes");
+                        multipliers, num_multipliers, widths, num_widths, true, out, out_params, nullptr, nullptr, nullptr,
+                        workspace, workspace_bytes, max_ctas, stream, "fqb200_clip_mse_grid_workspace_bytes");
 }
 
 // the requests fqb200_kmeans1d takes (argument errors as a message, nullptr when they are fine)

@@ -23,7 +23,7 @@ from . import int_quantization
 from . import ops
 from .statistics import refuse_bap_mse
 
-__all__ = ["IntQuantizer", "int_quantizer", "WeightMse", "best_candidates", "refuse_clip_weight"]
+__all__ = ["IntQuantizer", "int_quantizer", "MseCandidates", "WeightMse", "best_candidates", "refuse_clip_weight"]
 
 
 def _laplace_opt_alpha(w):
@@ -93,29 +93,37 @@ def best_candidates(err):
     return pick, err.gather(2, pick.unsqueeze(2)).squeeze(2)
 
 
-class WeightMse(object):
-    """What `clip_weight="mse"` shares across one model's weight quantizers: the float32 clipping multipliers and their
-    prior ("laplace": alpha = m * b, "gaus": m * std), their device copies, the int32 device flag fqb200_allocate_widths
-    raises on non-finite error tables, and with ``report`` (a CSV path) one row of device sums per quantized weight.
-    Nothing is read back until ``finish``, which reads the flag and the report in one copy."""
+class MseCandidates(object):
+    """The clipping candidates of measured clipping, shared by one model's quantizers: the float32 multipliers and their
+    prior ("laplace": alpha = m * b, "gaus": m * std), with one device copy per device."""
+
+    def __init__(self, multipliers, prior):
+        self.multipliers = np.asarray(multipliers, dtype=np.float32).reshape(-1)
+        self.prior = prior
+        self._mult = {}
+
+    def mult(self, dev):
+        m = self._mult.get(dev)
+        if m is None:   # pinned and asynchronous: no host synchronisation inside quantize_model or a forward
+            m = self._mult[dev] = torch.from_numpy(self.multipliers).pin_memory().to(dev, non_blocking=True)
+        return m
+
+
+class WeightMse(MseCandidates):
+    """What `clip_weight="mse"` shares across one model's weight quantizers: the clipping candidates
+    (``MseCandidates``), the int32 device flag fqb200_allocate_widths raises on non-finite error tables, and with
+    ``report`` (a CSV path) one row of device sums per quantized weight.  Nothing is read back until ``finish``, which
+    reads the flag and the report in one copy."""
 
     REPORT_COLUMNS = ("id", "rows", "bits", "mse_minmax", "mse_chosen", "kept_minmax", "bits_minmax_alloc",
                       "mse_minmax_alloc")
 
     def __init__(self, multipliers, prior, report=None):
-        self.multipliers = np.asarray(multipliers, dtype=np.float32).reshape(-1)
-        self.prior = prior
+        super(WeightMse, self).__init__(multipliers, prior)
         self.report = report
-        self._mult = {}
         self._status = None
         self._rows = []   # (id, rows, numel, float64 device [6]: bits, sse min/max, sse chosen, kept, bits / sse of the
                           # min/max-only allocation)
-
-    def mult(self, dev):
-        m = self._mult.get(dev)
-        if m is None:   # pinned and asynchronous: no host synchronisation inside quantize_model
-            m = self._mult[dev] = torch.from_numpy(self.multipliers).pin_memory().to(dev, non_blocking=True)
-        return m
 
     def status(self, dev):
         if self._status is None:
@@ -147,6 +155,18 @@ class WeightMse(object):
         if bad:
             raise ValueError("clip_weight='mse': a weight's error table holds NaN or Inf, so its width allocation is not "
                              "defined (bit_alloc.allocate refuses such tables)")
+
+
+# `-c mse` on the fly without candidates from a manager (a bare quantizer): statistics.MSE_MULTIPLIERS times the Laplace b
+_DEFAULT_MSE_CANDIDATES = None
+
+
+def _default_mse_candidates():
+    global _DEFAULT_MSE_CANDIDATES
+    if _DEFAULT_MSE_CANDIDATES is None:
+        from .statistics import MSE_MULTIPLIERS
+        _DEFAULT_MSE_CANDIDATES = MseCandidates(MSE_MULTIPLIERS, "laplace")
+    return _DEFAULT_MSE_CANDIDATES
 
 
 # A call site's `-sm use` parameters: per channel, [C] delta / offset and the widths (or None) of the torch leaf; per
@@ -200,6 +220,9 @@ class IntQuantizer(object):
         # min/max range and the clipping candidates of ``weight_mse`` (a WeightMse)
         self.clip_weight = "no"
         self.weight_mse = None
+        # `-c mse` on the fly (no statistics manager): the MseCandidates each activation is measured over (set by the
+        # manager; None: statistics.MSE_MULTIPLIERS with the Laplace prior)
+        self.mse_candidates = None
         self._stat_cache = {}  # offline-statistics parameters are constants of a layer: solved once, kept on the device
         self.force_positive = False
         self.half_range = False
@@ -212,6 +235,7 @@ class IntQuantizer(object):
         self.export_stats = False
         self.last_stats = None
         self.last_weight_mse = None   # ... and of the most recent `clip_weight="mse"` weight (see _clip_mse_weights)
+        self.last_clip_choice = None  # ... and the [groups] chosen columns of the most recent `-c mse` on-the-fly call
         # per-call inputs of ``__call__``'s extensions (reset when the call returns)
         self._relu_follows, self._bca, self._residual, self._defer, self._pool, self._into = False, None, None, False, None, None
 
@@ -259,7 +283,7 @@ class IntQuantizer(object):
         self._into = out
         try:
             self._unsupported(stat_id)
-            if bias is not None and not self._bias_fusable(tensor):
+            if bias is not None and not self._bias_fusable(tensor, stat_id):
                 # what the convolution would have added (in place when the caller gave the tensor up)
                 b = bias.view((1, -1) + (1,) * (tensor.dim() - 2))
                 tensor = tensor.add_(b) if self.inplace else tensor + b
@@ -310,10 +334,13 @@ class IntQuantizer(object):
     def _positive(self):
         return bool(self.force_positive or self.half_range)
 
-    def _bias_fusable(self, tensor):
+    def _bias_fusable(self, tensor, stat_id=None):
         """Where the kernel can add the convolution bias itself: the per-channel activation layouts (channel = group)
-        and the per-tensor / per-sample min-max layouts of 4-D tensors with H*W % 4 == 0 (bias_period = H*W)."""
+        and the per-tensor / per-sample min-max layouts of 4-D tensors with H*W % 4 == 0 (bias_period = H*W).  Not `-c mse`
+        on the fly: its candidate sums have no bias operand (adding it first is the same single fp32 rounding)."""
         if self.kld or self.mtd_quant and not self._pc_act(tensor):
+            return False
+        if self.clipping == "mse" and stat_id is None and not self.mtd_quant:
             return False
         if (self.clipping != "no" or not self.pcq_w) and self._pc_act(tensor) and tensor.shape[1] > 1:
             return True
@@ -378,8 +405,9 @@ class IntQuantizer(object):
         out_q += (out_q > 0).to(out_q.dtype) * q_bias.view(1, -1, 1, 1)
         return out_q
 
-    def _quantize1(self, tensor, delta, offset, bits=None, layout=None, bias=None):
-        """Mode A launch; with ``bias_correct`` set the activation bias correction rides along."""
+    def _quantize1(self, tensor, delta, offset, bits=None, layout=None, bias=None, table=None):
+        """Mode A launch; with ``bias_correct`` set the activation bias correction rides along.  ``table``: the [C, 12]
+        parameter table of (delta, offset, bits) when the caller has it (a deferred shortcut hands it on)."""
         if self._bca is None or tensor.dim() != 4:
             # per-channel parameters of a channels-last tensor that the descriptor entry point takes as it is
             if ((self._defer or self._residual is not None or self._pool is not None or self._into is not None) and layout is not None
@@ -388,7 +416,7 @@ class IntQuantizer(object):
                 if self._defer:
                     # nothing to launch at all: the call that takes the tensor as its residual gets the leaf parameters as
                     # the table a stats_only launch would have exported (columns 8..11)
-                    tensor._fq_deferred = (self._given_table(delta, offset, bits), bias)
+                    tensor._fq_deferred = (table if table is not None else self._given_table(delta, offset, bits), bias)
                     return tensor
                 # the same leaf through the descriptor entry point, which can also finish a ResNet block / pool (`-sm use`)
                 return self._launch(tensor, layout, channels_last=True, range_mode=L.RANGE_GIVEN, leaf=L.LEAF_TORCH,
@@ -472,7 +500,7 @@ class IntQuantizer(object):
 
     def _fused(self, tensor, layout, **kw):
         """ops.fused, keeping the exported statistics table when ``export_stats`` is set."""
-        if not self.export_stats:
+        if not self.export_stats or kw.get("range_mode") == L.RANGE_GIVEN:   # given parameters: nothing to export
             return ops.fused(tensor, layout, **kw)
         res, self.last_stats = ops.fused(tensor, layout, want_stats=True, **kw)
         return res
@@ -657,12 +685,14 @@ class IntQuantizer(object):
         widths = allocate(mse, self.bit_alloc_target_act)
         return scale * m[np.arange(scale.size), widths], torch.tensor(widths, dtype=torch.float32, device=dev)
 
-    def _use_apply(self, p, tensor, bias):
-        """The one launch of use-mode parameters ``p``: per channel ``_quantize1``; per tensor the bias first (in place
-        when the caller gave the tensor up), the `-bca` fallback, the empty-range pass-through of the compiled leaf, then
-        ops.quantize1 (torch leaf) or ops.float2gemmlowp (compiled leaf)."""
+    def _use_apply(self, p, tensor, bias, table=None):
+        """The one launch of use-mode parameters ``p``: per channel ``_quantize1`` (``table``: their parameter table, if
+        the caller has it); per tensor the bias first (in place when the caller gave the tensor up), the `-bca` fallback,
+        the empty-range pass-through of the compiled leaf, then ops.quantize1 (torch leaf) or ops.float2gemmlowp
+        (compiled leaf)."""
         if p.per_channel:
-            return self._quantize1(tensor, p.delta, p.offset, bits=p.bits, layout=self._nchw_layout(tensor), bias=bias)
+            return self._quantize1(tensor, p.delta, p.offset, bits=p.bits, layout=self._nchw_layout(tensor), bias=bias,
+                                   table=table)
         bca = self._bca is not None and tensor.dim() == 4
         if p.preserve_zero is None and bca:
             return self._quantize1(tensor, p.delta, p.offset, bias=bias)   # one parameter set, per-channel correction
@@ -685,6 +715,8 @@ class IntQuantizer(object):
         self._unsupported(stat_id)
         if stat_id is not None:
             return self._use_apply(self._use_params(tensor, stat_id, clip_type), tensor, bias)
+        if clip_type == "mse":
+            return self._fly_mse(tensor, bias)
         mode, k = self._range_mode(clip_type)
         if self._pc_act(tensor) and tensor.shape[1] > 1:
             hist = self._hist(tensor)  # the reference measures entropy in gemmlowpQuantizeActivationPerChannel (:442-445)
@@ -699,6 +731,41 @@ class IntQuantizer(object):
         return self._fused(tensor, (1, 1, tensor.numel()), scope=L.SCOPE_GROUP, range_mode=mode, clip_k=k,
                          leaf=L.LEAF_TORCH, num_bits=self.num_bits, positive=self._positive(), solve_f64=True,
                          out=self._out(tensor), any_dense_format=True)
+
+    def _fly_mse(self, tensor, bias, max_ctas=0):
+        """`-c mse` on the fly: each group (channel, as the on-the-fly ACIQ launch quantizes per channel, else the whole
+        tensor) is clipped at the minimum of its own clipping-MSE curve over ``mse_candidates``.  A statistics-only launch
+        configured like the ACIQ launch (scope, ``positive``, `-baa` widths), one ops.clip_mse_select launch pair that
+        measures every candidate at the group's width and picks on the device, then the use-mode apply of the chosen
+        parameters (``_use_apply``: block epilogue, deferred shortcut, pooling, slice write and `-bca` as in `-sm use`).
+        ``bias`` is None: ``_bias_fusable`` has it added first.  Nothing goes through ``_stat_cache`` or back to the host."""
+        if self.measure_entropy:
+            raise NotImplementedError("-c mse on the fly does not measure entropy (-me): use -sm use with collected curves")
+        cand = self.mse_candidates or _default_mse_candidates()
+        positive = self._positive()
+        if self._pc_act(tensor) and tensor.shape[1] > 1:
+            layout = self._nchw_layout(tensor)
+            cl = ops.cl_eligible(tensor)
+            x = tensor if cl else tensor.contiguous()
+            alloc = self._allocates(True)
+            table = ops.fused(x, layout, stats_only=True, channels_last=cl, num_bits=self.num_bits, positive=positive,
+                              bit_alloc=self.bit_alloc_act, bit_alloc_prior=self._prior(),
+                              bit_alloc_round=self.bit_alloc_round, bit_alloc_target=self.bit_alloc_target_act)
+            _, choice, given, chosen = ops.clip_mse_select(x, table, layout, cl, self.num_bits, positive,
+                                                           cand.mult(tensor.device), prior=cand.prior, bit_alloc=alloc,
+                                                           solve_f64=False, max_ctas=max_ctas)
+            p = _UseParams(True, given[0], given[1], given[2] if alloc else None, None)
+        else:
+            x = tensor if ops.dense(tensor) else tensor.contiguous()
+            layout = (1, 1, x.numel())
+            table = ops.fused(x, layout, stats_only=True, num_bits=self.num_bits, positive=positive, any_dense_format=True)
+            _, choice, given, chosen = ops.clip_mse_select(x, table, layout, False, self.num_bits, positive,
+                                                           cand.mult(tensor.device), prior=cand.prior, solve_f64=True,
+                                                           max_ctas=max_ctas)
+            p = _UseParams(False, given[0, 0], given[1, 0], None, None)
+        if self.export_stats:
+            self.last_stats, self.last_clip_choice = chosen, choice
+        return self._use_apply(p, tensor, bias, table=chosen)
 
     def gemmlowpMinMaxQuantize(self, tensor, tag="", stat_id=None, weight_correction=None, bias=None):
         """Per-tensor min/max range through the compiled-leaf arithmetic, int_quantizer.py:361-379 + :605-614.

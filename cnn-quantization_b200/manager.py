@@ -36,7 +36,8 @@ def make_args(**over):
     mse_* / cos_* columns of `-sm collect`; the name of the reference's StatisticManager argument), ``collect_mse`` (also
     write the clipping-MSE curve of every call site's quantizer in `-sm collect`, over ``mse_multipliers`` - default
     statistics.MSE_MULTIPLIERS, 0.5 .. 16 in steps of 0.125 - times the Laplace b or, with ``mse_prior="gaus"``, the std;
-    `-c mse` in use mode clips at the minimum of those curves), ``collect_bits`` (also write, for every call site `-sm use`
+    `-c mse` in use mode clips at the minimum of those curves, and with ``stats_mode="no"`` each activation at the minimum
+    of its own curve over the same candidates, measured in every forward), ``collect_bits`` (also write, for every call site `-sm use`
     quantizes per channel with bit allocation, the error of its quantizer on each channel at every width 0..8; needs
     ``per_channel_quant_act``, ``bit_alloc_act`` and clipping laplace, gaus or no; ``bit_alloc_prior="mse"`` (`-bap mse`) then allocates the
     widths that minimise the sum of those errors, and allocates weight widths from the weights' own errors.  With
@@ -397,7 +398,7 @@ class QuantizationManagerInference(object):
         # The noise kind also measures the tensor the quantizer was handed, so activations are quantized out of place and
         # that tensor survives the launch; the convolution bias stays fused and is passed to the measurement.
         # `clip_weight="mse"`: measured clipping of the per-channel weights, shared by the weight quantizers
-        from .int_quantizer import WeightMse, refuse_clip_weight
+        from .int_quantizer import MseCandidates, WeightMse, refuse_clip_weight
         clip_weight = getattr(args, "clip_weight", "no")
         refuse_clip_weight(clip_weight, args.per_channel_quant_weights, args.mid_thread_quant, qweight=args.qweight,
                            native=self._native)
@@ -409,6 +410,16 @@ class QuantizationManagerInference(object):
             from .statistics import _mse_multipliers
             prior = getattr(args, "mse_prior", "laplace")
             self.weight_mse = WeightMse(_mse_multipliers(getattr(args, "mse_multipliers", None), prior), prior, report)
+        # `-c mse` with on-the-fly statistics: every activation is clipped at the minimum of its own clipping-MSE curve
+        # over these candidates, measured and chosen on the device in each forward
+        self.fly_mse = None
+        if args.clipping == "mse" and self.stats_mode == "no":
+            from .statistics import _mse_multipliers
+            prior = getattr(args, "mse_prior", "laplace")
+            self.fly_mse = MseCandidates(_mse_multipliers(getattr(args, "mse_multipliers", None), prior), prior)
+            if args.measure_entropy and not getattr(args, "mid_thread_quant", False):
+                raise NotImplementedError("-c mse with -sm no does not measure entropy (-me): use -sm use with curves "
+                                          "collected with collect_mse=True")
         self.measure_stats = None
         kind = getattr(args, "measure_stats_kind", "distance")
         if kind not in ("distance", "angle", "noise"):
@@ -519,6 +530,10 @@ class QuantizationManagerInference(object):
             if self.weight_mse is not None:
                 for tag in ("weight", "weight_classifier"):
                     self.quantizers[tag].clip_weight, self.quantizers[tag].weight_mse = "mse", self.weight_mse
+            if self.fly_mse is not None:
+                for q in list(self.quantizers.values()) + [self.quantizer_default]:
+                    if getattr(q, "clipping", None) == "mse":
+                        q.mse_candidates = self.fly_mse
             if self.stats_mode == "use":
                 # which statistics each tag reads (IntQuantizer.__init__ :88 + the overrides of __fill_quantizers__)
                 per_tensor = lambda: self._sm_tensor

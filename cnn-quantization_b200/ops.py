@@ -25,8 +25,8 @@ def profile_collect():
     traffic: 'D' two statistics passes + apply (16 B/elem), 'B' one statistics pass + apply (12), 'A' apply only (8),
     'S' statistics only; 'K' the KLD calibration (ops.kld_threshold), 'M' the activation norm measurement
     (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'N' the quantization-noise measurement
-    (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error), 'R' the clipping-MSE curves (ops.clip_mse)
-    and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing; 'W' the given-parameter
+    (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error), 'R' the clipping-MSE curves (ops.clip_mse,
+    and with the choice of each group's clipping value ops.clip_mse_select) and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing; 'W' the given-parameter
     weight launch with its corrections (ops.quantize_weights_given) and 'L' the width allocation (ops.allocate_widths)."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
@@ -674,6 +674,31 @@ def clip_mse(x, table, layout, channels_last, num_bits, positive, multipliers, p
         else:
             _launch(x.device, timed, lib.fqb200_clip_mse_widths, *head, widths.ctypes.data, *tail)
     return (out, params) if want_params else out
+
+
+def clip_mse_select(x, table, layout, channels_last, num_bits, positive, multipliers, prior="laplace", bit_alloc=False,
+                    solve_f64=None, max_ctas=0):
+    """C ABI fqb200_clip_mse_select: ``clip_mse`` (same arguments, prior "laplace" or "gaus") together with each group's
+    choice, made on the device without a host round trip - `-c mse` on the fly.  Returns (sums, choice, given, table):
+    the [groups, K + 1] float64 sums of ``clip_mse``, bit for bit; the int32 [groups] column of the least error in
+    statistics.best_columns' order (ties: the smaller multiplier; NaN never wins); the float32 [3, groups] delta, offset
+    and bits of that candidate, bit for bit ``clip_mse``'s parameters at that column; and the float32 [groups, 12]
+    parameter table (``_lib.STAT_COLUMNS``: ``table``'s statistics, then the chosen candidate's parameters and torch
+    leaf).  Recorded in the launch profile under mode 'R' (one read of the tensor)."""
+    x, table, mult, (outer, groups, inner), solve_f64, out, _ = _clip_io(
+        "clip_mse_select", x, table, layout, channels_last, solve_f64, False, 1, multipliers,
+        prior not in ("laplace", "gaus") and "clip_mse_select: prior must be 'laplace' or 'gaus', got %r" % (prior,))
+    k = mult.numel()
+    choice = torch.empty(groups, dtype=torch.int32, device=x.device)
+    given = torch.empty((3, groups), dtype=torch.float32, device=x.device)
+    chosen = torch.empty((groups, L.STATS_STRIDE), dtype=torch.float32, device=x.device)
+    lib = L.load()
+    ws = _own_workspace(x.device, lib.fqb200_clip_mse_workspace_bytes(outer, groups, inner, int(bool(channels_last)), k))
+    _launch(x.device, _Timed("R", x.numel(), 4, "%dx%dx%d" % (outer, groups, inner)), lib.fqb200_clip_mse_select,
+            x.data_ptr(), outer, groups, inner, int(bool(channels_last)), table.data_ptr(), int(num_bits), int(bool(positive)),
+            int(bool(bit_alloc)), int(bool(solve_f64)), CLIP_MSE_PRIORS[prior], mult.data_ptr(), k, out.data_ptr(), None,
+            choice.data_ptr(), given.data_ptr(), chosen.data_ptr(), ws.data_ptr(), ws.numel(), int(max_ctas))
+    return out, choice, given, chosen
 
 
 def clip_mse_grid(x, table, layout, channels_last, num_bits, positive, multipliers, widths, prior="laplace", solve_f64=None,

@@ -403,8 +403,27 @@ int fqb200_clip_mse_widths(const float* in, int64_t outer, int64_t groups, int64
                            int32_t prior, const float* multipliers, const int32_t* widths, int32_t num_multipliers,
                            double* out, float* out_params, void* workspace, size_t workspace_bytes, int32_t max_ctas,
                            void* stream);
-/* Workspace of fqb200_clip_mse and fqb200_clip_mse_widths in bytes (0 and fqb200_last_error() on a layout or K it does not
- * take). */
+/*
+ * fqb200_clip_mse with the choice of each group's clipping value on the device (`-c mse` on the fly): the same `out`
+ * sums, bit for bit, and then, in the second launch once a group's sums are final, per group g:
+ *   choice[g]   (int32) the column k of the least sum (x - q_k)^2 in statistics.best_columns' order: ties go to the
+ *               smaller multiplier, then the earlier column; NaN never wins, so a row of NaN takes the smallest multiplier
+ *   given[g], given[groups + g], given[2 * groups + g]   (float32) that candidate's delta, offset and bits, bit for bit
+ *               out_params' values at column k
+ *   out_table (optional, [groups][FQB200_STATS_STRIDE] floats): columns 0..4 copied from `stats`, 5..10 the chosen
+ *               delta, offset, bits, scale, zero point and qmax of the torch leaf, 11 its flags - the table a deferred
+ *               shortcut hands to the launch that quantizes it.
+ * No atomics and no host synchronisation.  The arguments of fqb200_clip_mse (prior 0 or 1, no widths) and its workspace
+ * (fqb200_clip_mse_workspace_bytes).  FQB200_ERR_INVALID, before any CUDA call: fqb200_clip_mse's argument errors and a
+ * null choice or given.
+ */
+int fqb200_clip_mse_select(const float* in, int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
+                           const float* stats, int32_t num_bits, int32_t positive, int32_t bit_alloc, int32_t solve_f64,
+                           int32_t prior, const float* multipliers, int32_t num_multipliers, double* out, float* out_params,
+                           int32_t* choice, float* given, float* out_table, void* workspace, size_t workspace_bytes,
+                           int32_t max_ctas, void* stream);
+/* Workspace of fqb200_clip_mse, fqb200_clip_mse_widths and fqb200_clip_mse_select in bytes (0 and fqb200_last_error() on
+ * a layout or K it does not take). */
 size_t fqb200_clip_mse_workspace_bytes(int64_t outer, int64_t groups, int64_t inner, int32_t channels_last,
                                        int32_t num_multipliers);
 /*
