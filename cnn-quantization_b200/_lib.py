@@ -92,6 +92,9 @@ PROTOTYPES = {
     "fqb200_quantize_weights_given_workspace_bytes": (_sz, [_i64, _i64, _i32, _i32, _i32, _i32]),
     "fqb200_allocate_widths": (_i32, [_vp, _i64, ctypes.c_double, _vp, _vp, _vp, _sz, _vp]),
     "fqb200_allocate_widths_workspace_bytes": (_sz, [_i64, ctypes.c_double]),
+    "fqb200_allocate_select": (_i32, [_vp, _vp, _vp, _i32, _vp, _i64, ctypes.c_double, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                      _vp]),
+    "fqb200_allocate_select_workspace_bytes": (_sz, [_i64, ctypes.c_double]),
 }
 SYMBOLS = tuple(PROTOTYPES)
 

@@ -3012,6 +3012,59 @@ int fqb200_allocate_widths(const double* sse, int64_t groups, double target, flo
   return launched("fq_allocate_widths_kernel");
 }
 
+// fqb200_allocate_select's workspace: the per-width least sums [G][9] (float64) and their columns [G][9] (uint8), then
+// fqb200_allocate_widths' choice table and rows
+static size_t alloc_select_head(int64_t groups) {
+  return static_cast<size_t>(groups) * 9u * sizeof(double) + ((static_cast<size_t>(groups) * 9u + 15u) & ~static_cast<size_t>(15u));
+}
+
+size_t fqb200_allocate_select_workspace_bytes(int64_t groups, double target) {
+  g_err[0] = 0;
+  const size_t dp = fqb200_allocate_widths_workspace_bytes(groups, target);
+  return dp ? alloc_select_head(groups) + dp : 0u;
+}
+
+int fqb200_allocate_select(const double* sums, const float* out_params, const float* multipliers, int32_t num_multipliers,
+                           const float* stats, int64_t groups, double target, float* widths_out, int32_t* choice_out,
+                           float* given, float* out_table, int32_t* status, void* workspace, size_t workspace_bytes,
+                           void* stream) {
+  g_err[0] = 0;
+  const char* bad = alloc_bad_args(groups, target);
+  if (bad) return fail(FQB200_ERR_INVALID, bad);
+  if (num_multipliers < 1 || num_multipliers > fqb::kCmMaxK) return fail(FQB200_ERR_INVALID, "num_multipliers must be in 1..256%s");
+  if (!sums || !out_params || !widths_out || !given || (num_multipliers > 1 && !multipliers) || (out_table && !stats))
+    return fail(FQB200_ERR_INVALID, "null pointer%s");
+  const int64_t budget = alloc_budget(groups, target);
+  const bool in_smem = alloc_rows_in_smem(budget);
+  int rc = check_workspace(workspace, workspace_bytes, fqb200_allocate_select_workspace_bytes(groups, target),
+                           "fqb200_allocate_select_workspace_bytes");
+  if (rc != FQB200_OK) return rc;
+  const size_t smem = in_smem ? 2u * static_cast<size_t>(budget + 1) * sizeof(double) : 0u;
+  cudaError_t e = setup(fqb::fq_allocate_select_kernel, fqb::kAllocThreads, smem);
+  if (e != cudaSuccess) return fail(FQB200_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  fqb::AllocSelectArgs A;
+  memset(&A, 0, sizeof(A));
+  A.sums = sums;
+  A.params = out_params;
+  A.mult = multipliers;
+  A.stats = stats;
+  A.groups = static_cast<unsigned>(groups);
+  A.budget = static_cast<unsigned>(budget);
+  A.M = num_multipliers;
+  A.least = reinterpret_cast<double*>(ws);
+  A.column = ws + static_cast<size_t>(groups) * 9u * sizeof(double);
+  A.choice = ws + alloc_select_head(groups);
+  A.rows = in_smem ? nullptr : reinterpret_cast<double*>(A.choice + alloc_choice_bytes(groups, budget));
+  A.widths = widths_out;
+  A.chosen = choice_out;
+  A.given = given;
+  A.table = out_table;
+  A.status = status;
+  fqb::fq_allocate_select_kernel<<<1, fqb::kAllocThreads, smem, static_cast<cudaStream_t>(stream)>>>(A);
+  return launched("fq_allocate_select_kernel");
+}
+
 int fqb200_selftest_division(const float* a, const float* b, float* fast, float* ieee, int64_t n, void* stream) {
   if (n <= 0) return FQB200_OK;
   fqb::fq_divtest_kernel<<<296, 256, 0, static_cast<cudaStream_t>(stream)>>>(a, b, fast, ieee, static_cast<unsigned long long>(n));

@@ -169,6 +169,19 @@ def _default_mse_candidates():
     return _DEFAULT_MSE_CANDIDATES
 
 
+# `-baa -bap mse` on the fly: the width candidates of statistics.bit_candidates per (rule, positive, num_bits), constants
+_BIT_CANDIDATES = {}
+
+
+def _bit_candidates(rule, positive, num_bits):
+    key = (rule, bool(positive), num_bits)
+    cand = _BIT_CANDIDATES.get(key)
+    if cand is None:
+        from .statistics import bit_candidates
+        cand = _BIT_CANDIDATES[key] = MseCandidates(*bit_candidates(rule, positive, num_bits))
+    return cand
+
+
 # A call site's `-sm use` parameters: per channel, [C] delta / offset and the widths (or None) of the torch leaf; per
 # tensor, 0-d delta / offset of the torch leaf (preserve_zero None), or the float range / offset and preserve_zero of the
 # compiled leaf, whose range is None where the tensor passes through unquantized.
@@ -223,6 +236,9 @@ class IntQuantizer(object):
         # `-c mse` on the fly (no statistics manager): the MseCandidates each activation is measured over (set by the
         # manager; None: statistics.MSE_MULTIPLIERS with the Laplace prior)
         self.mse_candidates = None
+        # `-baa -bap mse` on the fly (no statistics manager, set by the manager with fly_bits): each per-channel,
+        # bit-allocated activation gets the widths that minimise the sum of its own per-channel errors, in every forward
+        self.fly_bits = False
         self._stat_cache = {}  # offline-statistics parameters are constants of a layer: solved once, kept on the device
         self.force_positive = False
         self.half_range = False
@@ -342,6 +358,8 @@ class IntQuantizer(object):
             return False
         if self.clipping == "mse" and stat_id is None and not self.mtd_quant:
             return False
+        if stat_id is None and self._fly_bits_site(tensor):   # the same: its candidate sums have no bias operand
+            return False
         if (self.clipping != "no" or not self.pcq_w) and self._pc_act(tensor) and tensor.shape[1] > 1:
             return True
         minmax = self.clipping == "no" and not self.pcq_w and not self._pc_act(tensor)
@@ -389,6 +407,8 @@ class IntQuantizer(object):
     def _prior(self):
         """The prior of the on-the-fly activation launches' bit allocation."""
         if self.bit_alloc_prior == "mse":
+            if self.fly_bits and not self._allocates(True):
+                return L.PRIOR_B   # above 4 bits nothing is allocated (the launch reads no prior); fly_bits takes the rest
             refuse_bap_mse(needs_use=self.bit_alloc_act)
         return L.PRIOR_STD if self.bit_alloc_prior == "gaus" else L.PRIOR_B
 
@@ -514,6 +534,12 @@ class IntQuantizer(object):
     def _allocates(self, per_channel):
         """Whether a call site's activation channels get their own widths (int_quantizer.py:236-247, :430-438)."""
         return bool(self.bit_alloc_act and per_channel and self.num_bits <= 4)
+
+    def _fly_bits_site(self, tensor):
+        """Whether ``fly_bits`` allocates this activation on the fly: a per-channel (per-channel ACIQ needs C > 1),
+        bit-allocated call site of the clipping or min/max dispatch target."""
+        return bool(self.fly_bits and not self.kld and not self.mtd_quant and self._pc_act(tensor)
+                    and (self.clipping == "no" or tensor.shape[1] > 1) and self._allocates(True))
 
     def _use_bits(self, stat_id, per_channel, dev):
         """None, or the float32 [C] widths of a per-channel, bit-allocated call site from ``_stat_bits``."""
@@ -715,6 +741,8 @@ class IntQuantizer(object):
         self._unsupported(stat_id)
         if stat_id is not None:
             return self._use_apply(self._use_params(tensor, stat_id, clip_type), tensor, bias)
+        if self._fly_bits_site(tensor):
+            return self._fly_bits(tensor, bias, clip_type)
         if clip_type == "mse":
             return self._fly_mse(tensor, bias)
         mode, k = self._range_mode(clip_type)
@@ -767,6 +795,38 @@ class IntQuantizer(object):
             self.last_stats, self.last_clip_choice = chosen, choice
         return self._use_apply(p, tensor, bias, table=chosen)
 
+    def _fly_bits(self, tensor, bias, rule, max_ctas=0):
+        """`-baa -bap mse` on the fly (``fly_bits``): the channels of a per-channel, bit-allocated activation get the
+        widths that minimise the sum of their own measured errors for ``bit_alloc_target_act`` bits per channel, the
+        allocation `-sm use` makes from tables collected with collect_bits under clipping ``rule``.  A statistics-only
+        launch without allocation (every candidate brings its own width), the candidates of each width 0..8 - those of
+        statistics.bit_candidates through ops.clip_mse, or under -c mse every width times ``mse_candidates`` through
+        ops.clip_mse_grid - then one ops.allocate_select, and the use-mode apply of its parameters (``_use_apply``: block
+        epilogue, deferred shortcut, pooling, slice write and `-bca` as in `-sm use`).  ``bias`` is None: ``_bias_fusable``
+        has it added first.  Nothing goes through ``_stat_cache`` or back to the host."""
+        if self.measure_entropy:
+            raise NotImplementedError("-baa -bap mse on the fly (fly_bits) does not measure entropy (-me)")
+        positive = self._positive()
+        layout = self._nchw_layout(tensor)
+        cl = ops.cl_eligible(tensor)
+        x = tensor if cl else tensor.contiguous()
+        dev = tensor.device
+        table = ops.fused(x, layout, stats_only=True, channels_last=cl, num_bits=8)
+        if rule == "mse":
+            cand = self.mse_candidates or _default_mse_candidates()
+            mult = cand.mult(dev)
+            sums, params = ops.clip_mse_grid(x, table, layout, cl, self.num_bits, positive, mult, range(9),
+                                             prior=cand.prior, solve_f64=False, want_params=True, max_ctas=max_ctas)
+        else:
+            cand = _bit_candidates(rule, positive, self.num_bits)
+            mult = None
+            sums, params = ops.clip_mse(x, table, layout, cl, self.num_bits, positive, cand.mult(dev), prior=cand.prior,
+                                        widths=range(9), solve_f64=False, want_params=True, max_ctas=max_ctas)
+        _, choice, given, chosen = ops.allocate_select(sums, params, table, self.bit_alloc_target_act, multipliers=mult)
+        if self.export_stats:
+            self.last_stats, self.last_clip_choice = chosen, choice   # choice: None without a multiplier grid
+        return self._use_apply(_UseParams(True, given[0], given[1], given[2], None), tensor, bias, table=chosen)
+
     def gemmlowpMinMaxQuantize(self, tensor, tag="", stat_id=None, weight_correction=None, bias=None):
         """Per-tensor min/max range through the compiled-leaf arithmetic, int_quantizer.py:361-379 + :605-614.
         Activations (tag contains 'activation', not 'classifier') use the batch average of per-sample min/max."""
@@ -813,6 +873,8 @@ class IntQuantizer(object):
         layout = self._nchw_layout(tensor)
         if stat_id is not None and min_ is None and max_ is None:
             return self._use_apply(self._use_params(tensor, stat_id, "minmax_pc"), tensor, bias)
+        if min_ is None and max_ is None and self._fly_bits_site(tensor):
+            return self._fly_bits(tensor, bias, "no")
         if min_ is None and max_ is None:
             hist = self._hist(tensor)
             res = self._launch(tensor, layout, channels_last=ops.cl_eligible(tensor),

@@ -49,8 +49,12 @@ def make_args(**over):
     per-sample quantization error statistics of its measure_statistics module, which the reference cannot run),
     ``clip_weight`` ("no" or "mse": quantize each output channel of a per-channel weight at the least measured squared
     error among its min/max range and the ``mse_multipliers`` clipping values under ``mse_prior``, at the widths `-baw`
-    gives it or, with `-bap mse`, at the widths that minimise the sum of those least errors) and ``weight_mse_report`` (a
-    CSV path: one row per weight quantized under clip_weight "mse", written after quantize_model)."""
+    gives it or, with `-bap mse`, at the widths that minimise the sum of those least errors), ``weight_mse_report`` (a
+    CSV path: one row per weight quantized under clip_weight "mse", written after quantize_model) and ``fly_bits``
+    (`-baa -bap mse` with ``stats_mode="no"``: every per-channel, bit-allocated activation gets, in each forward, the
+    widths that minimise the sum of its own per-channel errors - the tables collect_bits would collect under the same
+    clipping rule, measured and allocated on the GPU; clipping laplace, gaus, no or mse, the last over ``mse_multipliers``
+    times ``mse_prior``'s scale)."""
     d = dict(arch="resnet18", qtype=None, qweight="int8", q_off=False, clipping="no", stats_mode="no", stats_kind="mean",
              stats_folder=None, stats_batch_avg=False, kld_threshold=False, measure_stats=False,
              per_channel_quant_weights=False, per_channel_quant_act=False, bit_alloc_act=False, bit_alloc_weight=False,
@@ -58,7 +62,7 @@ def make_args(**over):
              bias_corr_act=False, bias_corr_weight=False, var_corr_weight=False, measure_entropy=False,
              mid_thread_quant=False, rho_act=None, rho_weight=None, preserve_zero=False, stats_base_dir=None,
              collect_err=False, measure_stats_kind="distance", collect_mse=False, mse_multipliers=None, mse_prior="laplace",
-             collect_bits=False, clip_weight="no", weight_mse_report=None)
+             collect_bits=False, clip_weight="no", weight_mse_report=None, fly_bits=False)
     d.update(over)
     return argparse.Namespace(**d)
 
@@ -464,11 +468,28 @@ class QuantizationManagerInference(object):
                 raise ValueError("collect_bits measures the per-channel error tables of -sm collect: it needs %s"
                                  % ", ".join(missing))
         bap_mse = getattr(args, "bit_alloc_prior", None) == "mse"
+        # `fly_bits`: `-baa -bap mse` with on-the-fly statistics - each activation's tables measured and allocated on the
+        # device in every forward
+        self.fly_bits = bool(getattr(args, "fly_bits", False))
         if bap_mse:   # a k*std rule is refused by the quantizer, at the call sites that would allocate under it
             refuse_bap_mse(kld=args.kld_threshold, clipping="mix" if args.clipping == "mix" else None,
                            mid_tread=getattr(args, "mid_thread_quant", False),
-                           needs_use=args.bit_alloc_act and self.stats_mode == "no",
+                           needs_use=args.bit_alloc_act and self.stats_mode == "no" and not self.fly_bits,
                            collect=args.bit_alloc_act and (self.collect_err or self.collect_mse))
+        if self.fly_bits:
+            missing = [what for what, ok in (("stats_mode='no'", self.stats_mode == "no"),
+                                              ("a qtype", args.qtype is not None),
+                                              ("per_channel_quant_act", args.per_channel_quant_act),
+                                              ("bit_alloc_act", args.bit_alloc_act),
+                                              ("bit_alloc_prior='mse'", bap_mse),
+                                              ("clipping laplace, gaus, no or mse", args.clipping in BIT_RULES),
+                                              ("this package's quantizers (no quantizer_factory)", self._native))
+                       if not ok]
+            if missing:
+                raise ValueError("fly_bits allocates each activation's widths from its own per-channel error tables in "
+                                 "every forward: it needs %s" % ", ".join(missing))
+            if args.measure_entropy:
+                raise NotImplementedError("-baa -bap mse on the fly (fly_bits) does not measure entropy (-me)")
         self.bit_mse = None
         # offline statistics (inference_quantization_manager.py:299-318)
         self.stats_manager = None
@@ -534,6 +555,10 @@ class QuantizationManagerInference(object):
                 for q in list(self.quantizers.values()) + [self.quantizer_default]:
                     if getattr(q, "clipping", None) == "mse":
                         q.mse_candidates = self.fly_mse
+            if self.fly_bits:   # the quantizers take the route at the per-channel, bit-allocated activation call sites
+                for q in list(self.quantizers.values()) + [self.quantizer_default]:
+                    if hasattr(q, "fly_bits"):
+                        q.fly_bits = True
             if self.stats_mode == "use":
                 # which statistics each tag reads (IntQuantizer.__init__ :88 + the overrides of __fill_quantizers__)
                 per_tensor = lambda: self._sm_tensor

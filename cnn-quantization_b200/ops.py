@@ -27,7 +27,8 @@ def profile_collect():
     (ops.sample_sumsq), 'G' the sample-angle measurement (ops.sample_angles), 'N' the quantization-noise measurement
     (ops.sample_noise), 'E' the clipping-error measurement (ops.clip_error), 'R' the clipping-MSE curves (ops.clip_mse,
     and with the choice of each group's clipping value ops.clip_mse_select) and 'C' the k-means clustering of a weight tensor (ops.kmeans1d), which quantize nothing; 'W' the given-parameter
-    weight launch with its corrections (ops.quantize_weights_given) and 'L' the width allocation (ops.allocate_widths)."""
+    weight launch with its corrections (ops.quantize_weights_given) and 'L' the width allocation (ops.allocate_widths,
+    and from a call site's error sums to its parameters ops.allocate_select)."""
     torch.cuda.synchronize()
     modes, shapes = {}, {}
     for mode, elems, nbytes, e0, e1, tag in _prof["records"]:
@@ -781,6 +782,49 @@ def allocate_widths(sse, target, status=None):
     _launch(sse.device, _Timed("L", groups, 72), lib.fqb200_allocate_widths, sse.data_ptr(), groups, float(target),
             out.data_ptr(), _ptr(status), ws.data_ptr(), ws.numel())
     return out
+
+
+def allocate_select(sums, params, stats, target, multipliers=None, status=None):
+    """C ABI fqb200_allocate_select: measured bit allocation from one call site's error sums to its apply parameters on the
+    device, without a host round trip (`-baa -bap mse` on the fly).  ``sums`` / ``params``: the float64 [G, 1 + 9 M] sums
+    and [G, 9 M, 6] parameters of ``clip_mse(..., widths=range(9), want_params=True)`` (M = 1) or of ``clip_mse_grid`` over
+    widths 0..8 and the M ``multipliers`` (float32 device tensor, required when M > 1); ``stats``: the float32 [G, 12]
+    table the candidates were solved from.  Per channel and width the least column in statistics.best_columns' order, then
+    ``allocate_widths`` over those sums for ``target`` bits per channel.  Returns (widths, choice, given, table): float32 [G]
+    widths; int32 [G] column of the chosen width (None when M = 1); float32 [3, G] delta, offset and bits, bit for bit
+    ``params`` at the chosen (width, column); the float32 [G, 12] parameter table of ``clip_mse_select``.  ``status``: an
+    int32 device tensor set to 1 on a non-finite per-width sum.  Recorded in the launch profile under mode 'L'."""
+    if not (isinstance(sums, torch.Tensor) and sums.is_cuda and sums.dtype == torch.float64 and sums.dim() == 2
+            and sums.shape[1] > 1 and (sums.shape[1] - 1) % 9 == 0):
+        raise ValueError("allocate_select needs float64 [G, 1 + 9 M] CUDA sums")
+    groups, m = sums.shape[0], (sums.shape[1] - 1) // 9
+    dev = sums.device
+    if not (isinstance(params, torch.Tensor) and params.dtype == torch.float32 and params.device == dev
+            and tuple(params.shape) == (groups, 9 * m, 6)):
+        raise ValueError("params must be the float32 [%d, %d, 6] candidate parameters on the sums' device" % (groups, 9 * m))
+    if not (isinstance(stats, torch.Tensor) and stats.dtype == torch.float32 and stats.device == dev
+            and tuple(stats.shape) == (groups, L.STATS_STRIDE)):
+        raise ValueError("stats must be the float32 [%d, %d] statistics table on the sums' device" % (groups, L.STATS_STRIDE))
+    mult = None
+    if m > 1:
+        if not (isinstance(multipliers, torch.Tensor) and multipliers.dtype == torch.float32 and multipliers.device == dev
+                and multipliers.numel() == m):
+            raise ValueError("allocate_select: %d columns per width need the %d float32 multipliers on the sums' device"
+                             % (m, m))
+        mult = multipliers.contiguous()
+    if status is not None and (status.dtype != torch.int32 or status.device != dev):
+        raise ValueError("status must be an int32 tensor on the sums' device")
+    lib = L.load()
+    sums, params, stats = sums.contiguous(), params.contiguous(), stats.contiguous()
+    ws = _own_workspace(dev, lib.fqb200_allocate_select_workspace_bytes(groups, float(target)))
+    widths = torch.empty(groups, dtype=torch.float32, device=dev)
+    choice = torch.empty(groups, dtype=torch.int32, device=dev) if m > 1 else None
+    given = torch.empty((3, groups), dtype=torch.float32, device=dev)
+    table = torch.empty((groups, L.STATS_STRIDE), dtype=torch.float32, device=dev)
+    _launch(dev, _Timed("L", groups, 72 * m), lib.fqb200_allocate_select, sums.data_ptr(), params.data_ptr(), _ptr(mult),
+            m, stats.data_ptr(), groups, float(target), widths.data_ptr(), _ptr(choice), given.data_ptr(), table.data_ptr(),
+            _ptr(status), ws.data_ptr(), ws.numel())
+    return widths, choice, given, table
 
 
 KMeans1d =collections.namedtuple("KMeans1d", "labels centres inertia n_iter init_ids out out_bcorr")

@@ -517,6 +517,29 @@ int fqb200_allocate_widths(const double* sse, int64_t groups, double target, flo
                            void* workspace, size_t workspace_bytes, void* stream);
 /* Workspace of fqb200_allocate_widths in bytes (0 and fqb200_last_error() on arguments it does not take). */
 size_t fqb200_allocate_widths_workspace_bytes(int64_t groups, double target);
+/*
+ * Measured bit allocation on the fly (`-baa -bap mse` with `-sm no`): from the error sums of one call site to the
+ * parameters its apply launch takes, in one launch and without host synchronisation.  `sums` (device float64
+ * [G][1 + 9 M]) and `out_params` ([G][9 M][6]) are what fqb200_clip_mse_widths (M = 1, widths 0..8) or
+ * fqb200_clip_mse_grid (widths 0..8 times M multipliers) write: column 1 + w * M + k is width w at multiplier k.
+ *   1. per channel g and width w, the column k of the least sum in statistics.best_columns' order over `multipliers`
+ *      (device, M floats, read only when M > 1): ties go to the smaller multiplier, then the earlier column; NaN never wins
+ *   2. the widths of fqb200_allocate_widths over those per-width sums (the same programme, bit for bit bit_alloc.allocate),
+ *      written to widths_out[G] (float32); *status (optional) is set to 1 on a non-finite per-width sum
+ *   3. per channel, for its width w and that width's column k: choice_out[g] = k (optional, int32); given[g],
+ *      given[G + g], given[2 G + g] the delta, offset and bits of out_params at (g, w * M + k), bit for bit; out_table
+ *      (optional, [G][FQB200_STATS_STRIDE]) columns 0..4 copied from `stats` ([G][FQB200_STATS_STRIDE]), 5..10 that
+ *      delta, offset, bits, scale, zero point and qmax of the torch leaf, 11 its flags, as fqb200_clip_mse_select writes it.
+ * No atomics.  Workspace (fqb200_allocate_select_workspace_bytes, private to the call, no initialisation).
+ * FQB200_ERR_INVALID, before any CUDA call: fqb200_allocate_widths' argument errors, M outside 1..256, a null sums,
+ * out_params, widths_out or given, a null multipliers with M > 1, a null stats with out_table.
+ */
+int fqb200_allocate_select(const double* sums, const float* out_params, const float* multipliers, int32_t num_multipliers,
+                           const float* stats, int64_t groups, double target, float* widths_out, int32_t* choice_out,
+                           float* given, float* out_table, int32_t* status, void* workspace, size_t workspace_bytes,
+                           void* stream);
+/* Workspace of fqb200_allocate_select in bytes (0 and fqb200_last_error() on arguments it does not take). */
+size_t fqb200_allocate_select_workspace_bytes(int64_t groups, double target);
 
 #ifdef __cplusplus
 }
