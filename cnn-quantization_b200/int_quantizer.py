@@ -13,6 +13,7 @@ bias correction (``-bca``) and ``mix`` clipping (``-sm use`` only: the per-layer
 Gauss and Laplace by the mse_* statistics collected with ``collect_err``, then one apply-only launch).
 """
 import collections
+import functools
 import math
 
 import numpy as np
@@ -21,7 +22,7 @@ import torch
 from . import _lib as L
 from . import int_quantization
 from . import ops
-from .statistics import refuse_bap_mse
+from .statistics import ClipErrConfig, MseCandidates, _curve, _width_tables, refuse_bap_mse
 
 __all__ = ["IntQuantizer", "int_quantizer", "MseCandidates", "WeightMse", "best_candidates", "refuse_clip_weight"]
 
@@ -93,33 +94,18 @@ def best_candidates(err):
     return pick, err.gather(2, pick.unsqueeze(2)).squeeze(2)
 
 
-class MseCandidates(object):
-    """The clipping candidates of measured clipping, shared by one model's quantizers: the float32 multipliers and their
-    prior ("laplace": alpha = m * b, "gaus": m * std), with one device copy per device."""
-
-    def __init__(self, multipliers, prior):
-        self.multipliers = np.asarray(multipliers, dtype=np.float32).reshape(-1)
-        self.prior = prior
-        self._mult = {}
-
-    def mult(self, dev):
-        m = self._mult.get(dev)
-        if m is None:   # pinned and asynchronous: no host synchronisation inside quantize_model or a forward
-            m = self._mult[dev] = torch.from_numpy(self.multipliers).pin_memory().to(dev, non_blocking=True)
-        return m
-
-
-class WeightMse(MseCandidates):
-    """What `clip_weight="mse"` shares across one model's weight quantizers: the clipping candidates
-    (``MseCandidates``), the int32 device flag fqb200_allocate_widths raises on non-finite error tables, and with
-    ``report`` (a CSV path) one row of device sums per quantized weight.  Nothing is read back until ``finish``, which
-    reads the flag and the report in one copy."""
+class WeightMse(object):
+    """What `clip_weight="mse"` shares across one model's weight quantizers: the clipping candidates (``candidates``,
+    ``MseCandidates.of(multipliers, prior)``: the run's set, or one of its own), the int32 device flag
+    fqb200_allocate_widths raises on non-finite error tables, and with ``report`` (a CSV path) one row of device sums per
+    quantized weight.  Nothing is read back until ``finish``, which reads the flag and the report in one copy."""
 
     REPORT_COLUMNS = ("id", "rows", "bits", "mse_minmax", "mse_chosen", "kept_minmax", "bits_minmax_alloc",
                       "mse_minmax_alloc")
 
-    def __init__(self, multipliers, prior, report=None):
-        super(WeightMse, self).__init__(multipliers, prior)
+    def __init__(self, multipliers, prior="laplace", report=None):
+        self.candidates = MseCandidates.of(multipliers, prior)
+        self.multipliers, self.prior = self.candidates.multipliers, self.candidates.prior
         self.report = report
         self._status = None
         self._rows = []   # (id, rows, numel, float64 device [6]: bits, sse min/max, sse chosen, kept, bits / sse of the
@@ -157,29 +143,10 @@ class WeightMse(MseCandidates):
                              "defined (bit_alloc.allocate refuses such tables)")
 
 
-# `-c mse` on the fly without candidates from a manager (a bare quantizer): statistics.MSE_MULTIPLIERS times the Laplace b
-_DEFAULT_MSE_CANDIDATES = None
-
-
+@functools.lru_cache(maxsize=None)
 def _default_mse_candidates():
-    global _DEFAULT_MSE_CANDIDATES
-    if _DEFAULT_MSE_CANDIDATES is None:
-        from .statistics import MSE_MULTIPLIERS
-        _DEFAULT_MSE_CANDIDATES = MseCandidates(MSE_MULTIPLIERS, "laplace")
-    return _DEFAULT_MSE_CANDIDATES
-
-
-# `-baa -bap mse` on the fly: the width candidates of statistics.bit_candidates per (rule, positive, num_bits), constants
-_BIT_CANDIDATES = {}
-
-
-def _bit_candidates(rule, positive, num_bits):
-    key = (rule, bool(positive), num_bits)
-    cand = _BIT_CANDIDATES.get(key)
-    if cand is None:
-        from .statistics import bit_candidates
-        cand = _BIT_CANDIDATES[key] = MseCandidates(*bit_candidates(rule, positive, num_bits))
-    return cand
+    """The candidates of `-c mse` on the fly without candidates from a manager (a bare quantizer): the default options."""
+    return MseCandidates.of()
 
 
 # A call site's `-sm use` parameters: per channel, [C] delta / offset and the widths (or None) of the torch leaf; per
@@ -234,7 +201,7 @@ class IntQuantizer(object):
         self.clip_weight = "no"
         self.weight_mse = None
         # `-c mse` on the fly (no statistics manager): the MseCandidates each activation is measured over (set by the
-        # manager; None: statistics.MSE_MULTIPLIERS with the Laplace prior)
+        # manager; None: the defaults of MseCandidates.of)
         self.mse_candidates = None
         # `-baa -bap mse` on the fly (no statistics manager, set by the manager with fly_bits): each per-channel,
         # bit-allocated activation gets the widths that minimise the sum of its own per-channel errors, in every forward
@@ -411,6 +378,17 @@ class IntQuantizer(object):
                 return L.PRIOR_B   # above 4 bits nothing is allocated (the launch reads no prior); fly_bits takes the rest
             refuse_bap_mse(needs_use=self.bit_alloc_act)
         return L.PRIOR_STD if self.bit_alloc_prior == "gaus" else L.PRIOR_B
+
+    def clip_err_config(self, tensor, half_range):
+        """The statistics.ClipErrConfig of this quantizer's on-the-fly activation launch on ``tensor`` with the call's
+        ``half_range``: per channel where that launch is (``_pc_act`` and C > 1), bit allocation only there, and the
+        prior of ``_prior`` without its `-bap mse` refusal (PRIOR_B).  The collect measurements (collect_err, collect_mse,
+        collect_bits) and the on-the-fly routes of measured clipping measure the quantizer it describes."""
+        per_channel = self._pc_act(tensor) and tensor.shape[1] > 1
+        return ClipErrConfig(num_bits=self.num_bits, positive=bool(self.force_positive or half_range),
+                             per_channel=per_channel, bit_alloc=self._allocates(per_channel),
+                             bit_alloc_prior=L.PRIOR_STD if self.bit_alloc_prior == "gaus" else L.PRIOR_B,
+                             bit_alloc_round=bool(self.bit_alloc_round), bit_alloc_target=self.bit_alloc_target_act)
 
     @staticmethod
     def bias_correction_torch(out, out_q, relu_first):
@@ -762,34 +740,21 @@ class IntQuantizer(object):
 
     def _fly_mse(self, tensor, bias, max_ctas=0):
         """`-c mse` on the fly: each group (channel, as the on-the-fly ACIQ launch quantizes per channel, else the whole
-        tensor) is clipped at the minimum of its own clipping-MSE curve over ``mse_candidates``.  A statistics-only launch
-        configured like the ACIQ launch (scope, ``positive``, `-baa` widths), one ops.clip_mse_select launch pair that
-        measures every candidate at the group's width and picks on the device, then the use-mode apply of the chosen
-        parameters (``_use_apply``: block epilogue, deferred shortcut, pooling, slice write and `-bca` as in `-sm use`).
-        ``bias`` is None: ``_bias_fusable`` has it added first.  Nothing goes through ``_stat_cache`` or back to the host."""
+        tensor) is clipped at the minimum of its own clipping-MSE curve over ``mse_candidates``: the curve collect_mse
+        measures (statistics._curve, with ``clip_err_config``'s quantizer: scope, ``positive``, `-baa` widths) through
+        ops.clip_mse_select, which picks on the device, then the use-mode apply of the chosen parameters (``_use_apply``:
+        block epilogue, deferred shortcut, pooling, slice write and `-bca` as in `-sm use`).  ``bias`` is None:
+        ``_bias_fusable`` has it added first.  Nothing goes through ``_stat_cache`` or back to the host."""
         if self.measure_entropy:
             raise NotImplementedError("-c mse on the fly does not measure entropy (-me): use -sm use with collected curves")
+        cfg = self.clip_err_config(tensor, self.half_range)
+        if cfg.per_channel:
+            self._prior()   # `-baa -bap mse` without fly_bits refuses here, as on the per-channel ACIQ launch
         cand = self.mse_candidates or _default_mse_candidates()
-        positive = self._positive()
-        if self._pc_act(tensor) and tensor.shape[1] > 1:
-            layout = self._nchw_layout(tensor)
-            cl = ops.cl_eligible(tensor)
-            x = tensor if cl else tensor.contiguous()
-            alloc = self._allocates(True)
-            table = ops.fused(x, layout, stats_only=True, channels_last=cl, num_bits=self.num_bits, positive=positive,
-                              bit_alloc=self.bit_alloc_act, bit_alloc_prior=self._prior(),
-                              bit_alloc_round=self.bit_alloc_round, bit_alloc_target=self.bit_alloc_target_act)
-            _, choice, given, chosen = ops.clip_mse_select(x, table, layout, cl, self.num_bits, positive,
-                                                           cand.mult(tensor.device), prior=cand.prior, bit_alloc=alloc,
-                                                           solve_f64=False, max_ctas=max_ctas)
-            p = _UseParams(True, given[0], given[1], given[2] if alloc else None, None)
+        _, _, _, _, (_, choice, given, chosen) = _curve(tensor, cfg, cand, select=True, max_ctas=max_ctas)
+        if cfg.per_channel:
+            p = _UseParams(True, given[0], given[1], given[2] if cfg.bit_alloc else None, None)
         else:
-            x = tensor if ops.dense(tensor) else tensor.contiguous()
-            layout = (1, 1, x.numel())
-            table = ops.fused(x, layout, stats_only=True, num_bits=self.num_bits, positive=positive, any_dense_format=True)
-            _, choice, given, chosen = ops.clip_mse_select(x, table, layout, False, self.num_bits, positive,
-                                                           cand.mult(tensor.device), prior=cand.prior, solve_f64=True,
-                                                           max_ctas=max_ctas)
             p = _UseParams(False, given[0, 0], given[1, 0], None, None)
         if self.export_stats:
             self.last_stats, self.last_clip_choice = chosen, choice
@@ -798,31 +763,19 @@ class IntQuantizer(object):
     def _fly_bits(self, tensor, bias, rule, max_ctas=0):
         """`-baa -bap mse` on the fly (``fly_bits``): the channels of a per-channel, bit-allocated activation get the
         widths that minimise the sum of their own measured errors for ``bit_alloc_target_act`` bits per channel, the
-        allocation `-sm use` makes from tables collected with collect_bits under clipping ``rule``.  A statistics-only
-        launch without allocation (every candidate brings its own width), the candidates of each width 0..8 - those of
-        statistics.bit_candidates through ops.clip_mse, or under -c mse every width times ``mse_candidates`` through
-        ops.clip_mse_grid - then one ops.allocate_select, and the use-mode apply of its parameters (``_use_apply``: block
-        epilogue, deferred shortcut, pooling, slice write and `-bca` as in `-sm use`).  ``bias`` is None: ``_bias_fusable``
-        has it added first.  Nothing goes through ``_stat_cache`` or back to the host."""
+        allocation `-sm use` makes from tables collected with collect_bits under clipping ``rule``: the tables collect_bits
+        measures (statistics._width_tables, with ``clip_err_config``'s quantizer, per channel even with one channel: the
+        candidates of statistics.bit_candidates, or under -c mse every width times ``mse_candidates``), then one
+        ops.allocate_select, and the use-mode apply of its parameters (``_use_apply``: block epilogue, deferred shortcut,
+        pooling, slice write and `-bca` as in `-sm use`).  ``bias`` is None: ``_bias_fusable`` has it added first.  Nothing
+        goes through ``_stat_cache`` or back to the host."""
         if self.measure_entropy:
             raise NotImplementedError("-baa -bap mse on the fly (fly_bits) does not measure entropy (-me)")
-        positive = self._positive()
-        layout = self._nchw_layout(tensor)
-        cl = ops.cl_eligible(tensor)
-        x = tensor if cl else tensor.contiguous()
-        dev = tensor.device
-        table = ops.fused(x, layout, stats_only=True, channels_last=cl, num_bits=8)
-        if rule == "mse":
-            cand = self.mse_candidates or _default_mse_candidates()
-            mult = cand.mult(dev)
-            sums, params = ops.clip_mse_grid(x, table, layout, cl, self.num_bits, positive, mult, range(9),
-                                             prior=cand.prior, solve_f64=False, want_params=True, max_ctas=max_ctas)
-        else:
-            cand = _bit_candidates(rule, positive, self.num_bits)
-            mult = None
-            sums, params = ops.clip_mse(x, table, layout, cl, self.num_bits, positive, cand.mult(dev), prior=cand.prior,
-                                        widths=range(9), solve_f64=False, want_params=True, max_ctas=max_ctas)
-        _, choice, given, chosen = ops.allocate_select(sums, params, table, self.bit_alloc_target_act, multipliers=mult)
+        cfg = self.clip_err_config(tensor, self.half_range)._replace(per_channel=True)
+        cand = self.mse_candidates or _default_mse_candidates()
+        _, _, _, table, (sums, params) = _width_tables(tensor, cfg, rule, cand, want_params=True, max_ctas=max_ctas)
+        mult = cand.mult(tensor.device) if rule == "mse" else None   # the grid's multipliers: allocate_select picks one
+        _, choice, given, chosen = ops.allocate_select(sums, params, table, cfg.bit_alloc_target, multipliers=mult)
         if self.export_stats:
             self.last_stats, self.last_clip_choice = chosen, choice   # choice: None without a multiplier grid
         return self._use_apply(_UseParams(True, given[0], given[1], given[2], None), tensor, bias, table=chosen)
@@ -978,7 +931,7 @@ class IntQuantizer(object):
                           bit_alloc_target=self.bit_alloc_target_weight, stats_only=True)
         widths = list(range(9)) if alloc else [self.num_bits]
         nw = len(widths)
-        mult = wm.mult(dev)
+        mult = wm.candidates.mult(dev)
         m = mult.numel()
         grid, gp = ops.clip_mse_grid(tensor, table, layout, False, self.num_bits, False, mult, widths, prior=wm.prior,
                                      want_params=True, max_ctas=max_ctas)

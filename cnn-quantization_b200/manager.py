@@ -20,7 +20,6 @@ from itertools import count
 import torch
 import torch.nn as nn
 
-from . import _lib as L
 from .dummy_quantizer import DummyQuantizer
 from .int_quantizer import int_quantizer as _default_factory
 
@@ -402,25 +401,24 @@ class QuantizationManagerInference(object):
         # The noise kind also measures the tensor the quantizer was handed, so activations are quantized out of place and
         # that tensor survives the launch; the convolution bias stays fused and is passed to the measurement.
         # `clip_weight="mse"`: measured clipping of the per-channel weights, shared by the weight quantizers
-        from .int_quantizer import MseCandidates, WeightMse, refuse_clip_weight
+        from .int_quantizer import WeightMse, refuse_clip_weight
         clip_weight = getattr(args, "clip_weight", "no")
         refuse_clip_weight(clip_weight, args.per_channel_quant_weights, args.mid_thread_quant, qweight=args.qweight,
                            native=self._native)
         report = getattr(args, "weight_mse_report", None)
         if report is not None and clip_weight != "mse":
             raise ValueError("weight_mse_report reports the weights quantized under clip_weight='mse'")
+        # the clipping candidates (mse_multipliers / mse_prior) every measurement of this run shares: checked where the
+        # first one needs them (``_mse_candidates``)
+        self._mse_set = None
         self.weight_mse = None
         if clip_weight == "mse":
-            from .statistics import _mse_multipliers
-            prior = getattr(args, "mse_prior", "laplace")
-            self.weight_mse = WeightMse(_mse_multipliers(getattr(args, "mse_multipliers", None), prior), prior, report)
+            self.weight_mse = WeightMse(self._mse_candidates(), report=report)
         # `-c mse` with on-the-fly statistics: every activation is clipped at the minimum of its own clipping-MSE curve
         # over these candidates, measured and chosen on the device in each forward
         self.fly_mse = None
         if args.clipping == "mse" and self.stats_mode == "no":
-            from .statistics import _mse_multipliers
-            prior = getattr(args, "mse_prior", "laplace")
-            self.fly_mse = MseCandidates(_mse_multipliers(getattr(args, "mse_multipliers", None), prior), prior)
+            self.fly_mse = self._mse_candidates()
             if args.measure_entropy and not getattr(args, "mid_thread_quant", False):
                 raise NotImplementedError("-c mse with -sm no does not measure entropy (-me): use -sm use with curves "
                                           "collected with collect_mse=True")
@@ -510,13 +508,11 @@ class QuantizationManagerInference(object):
                                                           batch_avg=args.stats_batch_avg, base_dir=base)
                 if self.collect_mse:
                     from .statistics import ClipMseStatistics
-                    self.clip_mse = ClipMseStatistics(sf, getattr(args, "mse_multipliers", None),
-                                                      getattr(args, "mse_prior", "laplace"), base_dir=base)
+                    self.clip_mse = ClipMseStatistics(sf, self._mse_candidates(), base_dir=base)
                 if self.collect_bits:
                     from .statistics import BitMseStatistics
                     self.bit_mse = BitMseStatistics(sf, args.clipping, base_dir=base,
-                                                    multipliers=getattr(args, "mse_multipliers", None),
-                                                    prior=getattr(args, "mse_prior", "laplace"))
+                                                    multipliers=self._mse_candidates() if args.clipping == "mse" else None)
             else:
                 if bap_mse:   # read on first use: a missing layer raises KeyError naming collect_bits there
                     from .statistics import BitMseStatistics
@@ -577,6 +573,14 @@ class QuantizationManagerInference(object):
                 self.set_8bit_list(["conv%d_activation" % i for i in [0]])  # createTruncationManager, :334-340
 
     # -- quantizer table (TruncationOpManagerInference.__fill_quantizers__, :407-476) ----------------
+    def _mse_candidates(self):
+        """The run's statistics.MseCandidates of mse_multipliers / mse_prior, made and checked on first use."""
+        if self._mse_set is None:
+            from .statistics import MseCandidates
+            self._mse_set = MseCandidates.of(getattr(self.args, "mse_multipliers", None),
+                                             getattr(self.args, "mse_prior", "laplace"))
+        return self._mse_set
+
     def _load(self, qtype, qparams):
         name = qtype.rstrip("1234567890")
         if name != "int":
@@ -802,21 +806,16 @@ class QuantizationManagerInference(object):
         return measured
 
     def _clip_err(self, out, tag, stat_id, half_range, name):
-        """``save_tensor_stats`` kwargs of a collect call site: with collect_err, the settings of the quantizer
-        quantize_instant picks for the same call in `-sm use` (``tag``, the 8-bit ``ignored`` list, ``half_range``) on
-        this tensor ``out``: per channel when it would quantize it per channel, with bit allocation only then.  With
-        collect_mse, the call site's clipping-MSE curve is measured here, with the same settings (``name``: the
-        internal name save_tensor_stats records).  With collect_bits, a call site it would quantize per channel with bit
-        allocation also gets its per-channel error tables measured."""
+        """``save_tensor_stats`` kwargs of a collect call site: with collect_err, the settings (``clip_err_config``, at
+        most 8 bits) of the quantizer quantize_instant picks for the same call in `-sm use` (``tag``, the 8-bit
+        ``ignored`` list, ``half_range``) on this tensor ``out``.  With collect_mse, the call site's clipping-MSE curve
+        is measured here, with the same settings (``name``: the internal name save_tensor_stats records).  With
+        collect_bits, a call site it would quantize per channel with bit allocation also gets its per-channel error
+        tables measured."""
         if not (self.collect_err or self.collect_mse or self.collect_bits):
             return {}
-        from .statistics import ClipErrConfig
         q = self.get_quantizer("ignored" if stat_id in self.ignore_ids else tag)
-        per_channel = bool(q.pcq_a and out.dim() == 4 and (out.shape[2] > 1 or out.shape[3] > 1) and out.shape[1] > 1)
-        cfg = ClipErrConfig(num_bits=min(q.num_bits, 8), positive=bool(q.force_positive or half_range),
-                            per_channel=per_channel, bit_alloc=bool(per_channel and q.bit_alloc_act and q.num_bits <= 4),
-                            bit_alloc_prior=L.PRIOR_STD if q.bit_alloc_prior == "gaus" else L.PRIOR_B,
-                            bit_alloc_round=bool(q.bit_alloc_round), bit_alloc_target=q.bit_alloc_target_act)
+        cfg = q.clip_err_config(out, half_range)._replace(num_bits=min(q.num_bits, 8))
         if self.collect_mse:
             self.clip_mse.save_curve(out, name, stat_id, cfg)
         if self.collect_bits:

@@ -64,6 +64,7 @@ bit allocation (`collect_bits`): the error the call site's quantizer makes on ea
 It costs the same as ``ClipMseStatistics`` with 9 candidates.
 """
 import collections
+import functools
 import os
 import pickle
 import re
@@ -75,7 +76,8 @@ import torch
 from . import ops
 
 __all__ = ["StatisticManager", "StatisticManagerPerChannel", "MeasureStatistics", "AngleStatistics", "NoiseStatistics",
-           "ClipErrConfig", "ClipMseStatistics", "MSE_MULTIPLIERS", "BitMseStatistics", "bit_candidates", "default_base_dir"]
+           "ClipErrConfig", "ClipMseStatistics", "MSE_MULTIPLIERS", "MseCandidates", "BitMseStatistics", "bit_candidates",
+           "default_base_dir"]
 
 
 def default_base_dir():
@@ -97,10 +99,9 @@ def sorted_nicely(keys):
 
 _ERR_COLUMNS = ["mse_lowp", "mse_gaus", "mse_laplace", "cos_lowp", "cos_gaus", "cos_laplace"]
 
-# The use-mode quantizer of one call site, as far as the error candidates need it: its bit width, its positive range
-# (half_range / force_positive), whether it quantizes this tensor per channel (pcq_a on a 4-D tensor with H or W > 1 and
-# C > 1, int_quantizer.py:333, :343-344) and its bit allocation (per channel with num_bits <= 4 only; prior PRIOR_STD /
-# PRIOR_B).
+# The quantizer of one call site, as far as the measurements need it (IntQuantizer.clip_err_config): its bit width, its
+# positive range (half_range / force_positive), whether it quantizes this tensor per channel and its bit allocation (per
+# channel with num_bits <= 4 only; prior PRIOR_STD / PRIOR_B).
 ClipErrConfig = collections.namedtuple("ClipErrConfig", "num_bits positive per_channel bit_alloc bit_alloc_prior "
                                                         "bit_alloc_round bit_alloc_target")
 
@@ -108,20 +109,53 @@ ClipErrConfig = collections.namedtuple("ClipErrConfig", "num_bits positive per_c
 def _stats_table(t, cfg, channels_last):
     """(``t`` in the memory order the launches read, layout, channels-last flag, table) of the statistics-only launch of
     the quantizer ``cfg`` describes: per channel (with ``cfg``'s bit allocation) in place on a channels-last ``t`` when
-    ``channels_last`` allows it, else on the NCHW tensor; per tensor in any dense memory order."""
+    ``channels_last`` allows it, else on the NCHW tensor; per tensor in any dense memory order.  The candidate launches
+    read the statistics (columns 0..4) and, with bit allocation, the widths (column 7) of the table; without allocation
+    the table is solved at 8 bits."""
     if not cfg.per_channel:
         if not ops.dense(t):
             t = t.contiguous()
         layout = (1, 1, t.numel())
-        return t, layout, False, ops.fused(t, layout, stats_only=True, any_dense_format=True)
+        return t, layout, False, ops.fused(t, layout, positive=cfg.positive, stats_only=True, any_dense_format=True)
     n, c = t.shape[0], t.shape[1]
     layout = (n, c, t.numel() // (n * c))
     cl = channels_last and ops.cl_eligible(t, layout)
     if not cl:
         t = t.contiguous()
-    return t, layout, cl, ops.fused(t, layout, num_bits=cfg.num_bits if cfg.bit_alloc else 8, bit_alloc=cfg.bit_alloc,
-                                    bit_alloc_prior=cfg.bit_alloc_prior, bit_alloc_round=cfg.bit_alloc_round,
-                                    bit_alloc_target=cfg.bit_alloc_target, stats_only=True, channels_last=cl)
+    return t, layout, cl, ops.fused(t, layout, num_bits=cfg.num_bits if cfg.bit_alloc else 8, positive=cfg.positive,
+                                    bit_alloc=cfg.bit_alloc, bit_alloc_prior=cfg.bit_alloc_prior,
+                                    bit_alloc_round=cfg.bit_alloc_round, bit_alloc_target=cfg.bit_alloc_target,
+                                    stats_only=True, channels_last=cl)
+
+
+def _curve(t, cfg, cand, select=False, max_ctas=0):
+    """The clipping-MSE curve of the quantizer ``cfg`` describes on ``t`` over the candidates ``cand`` (an
+    MseCandidates), each at the group's width: ``_stats_table``'s (tensor, layout, channels-last flag, table) and the
+    result of the candidate launch - ops.clip_mse's sums, or with ``select`` ops.clip_mse_select's (sums, choice, given
+    parameters, parameter table).  What `collect_mse` accumulates and `-c mse` on the fly chooses from."""
+    t, layout, cl, table = _stats_table(t, cfg, True)
+    launch = ops.clip_mse_select if select else ops.clip_mse
+    return t, layout, cl, table, launch(t, table, layout, cl, cfg.num_bits, cfg.positive, cand.mult(t.device),
+                                        prior=cand.prior, bit_alloc=cfg.bit_alloc, solve_f64=not cfg.per_channel,
+                                        max_ctas=max_ctas)
+
+
+def _width_tables(t, cfg, rule, cand, want_params=False, max_ctas=0):
+    """The per-channel error tables of the quantizer ``cfg`` describes on ``t`` at every width 0..8 under the clipping
+    ``rule``: ``_stats_table``'s (tensor, layout, channels-last flag, table) of an 8-bit table without allocation (every
+    candidate brings its own width) and the result of the candidate launch - ops.clip_mse over the candidates of
+    ``bit_candidates``, or under rule "mse" ops.clip_mse_grid over widths 0..8 times ``cand`` (an MseCandidates; unused
+    under the other rules); with ``want_params`` (sums, parameters).  What `collect_bits` accumulates and `fly_bits`
+    allocates from."""
+    t, layout, cl, table = _stats_table(t, cfg._replace(bit_alloc=False), True)
+    if rule == "mse":
+        out = ops.clip_mse_grid(t, table, layout, cl, cfg.num_bits, cfg.positive, cand.mult(t.device), range(9),
+                                prior=cand.prior, solve_f64=False, want_params=want_params, max_ctas=max_ctas)
+    else:
+        widths = _width_candidates(rule, cfg.positive, cfg.num_bits)
+        out = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive, widths.mult(t.device), prior=widths.prior,
+                           widths=range(9), solve_f64=False, want_params=want_params, max_ctas=max_ctas)
+    return t, layout, cl, table, out
 
 
 def _clip_sums(t, cfg, per_sample_channel):
@@ -576,15 +610,37 @@ def best_multipliers(multipliers, mse):
     return np.asarray(multipliers, dtype=np.float32)[best_columns(multipliers, mse)]
 
 
-def _mse_multipliers(multipliers, prior):
-    """float32 ``multipliers`` (default MSE_MULTIPLIERS) of the clipping values alpha = m * b (``prior`` "laplace") or
-    m * std ("gaus"), after checking both."""
-    if prior not in ("gaus", "laplace"):
-        raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
-    m = np.asarray(MSE_MULTIPLIERS if multipliers is None else multipliers, dtype=np.float32).reshape(-1)
-    if not 1 <= m.size <= 256:
-        raise ValueError("mse_multipliers: 1..256 values, got %d" % m.size)
-    return m
+class MseCandidates(object):
+    """The clipping candidates of one measurement: the float32 ``multipliers`` and their ``prior`` (ops.clip_mse's:
+    alpha = m * b for "laplace", m * std for "gaus"), with one device copy per device.  A manager builds one set from
+    mse_multipliers / mse_prior (``of``) and shares it between every measurement of the run."""
+
+    def __init__(self, multipliers, prior):
+        self.multipliers = np.asarray(multipliers, dtype=np.float32).reshape(-1)
+        self.prior = prior
+        self._mult = {}
+
+    @classmethod
+    def of(cls, multipliers=None, prior="laplace"):
+        """``multipliers`` itself when it is an MseCandidates (a run's shared set), else the candidates of the options
+        mse_multipliers (default MSE_MULTIPLIERS) and mse_prior, after checking both."""
+        if isinstance(multipliers, cls):
+            return multipliers
+        if prior not in ("gaus", "laplace"):
+            raise ValueError("mse_prior must be one of ['gaus', 'laplace'], got %r" % (prior,))
+        cand = cls(MSE_MULTIPLIERS if multipliers is None else multipliers, prior)
+        if not 1 <= cand.multipliers.size <= 256:
+            raise ValueError("mse_multipliers: 1..256 values, got %d" % cand.multipliers.size)
+        return cand
+
+    def mult(self, dev):
+        m = self._mult.get(dev)
+        if m is None:
+            m = torch.from_numpy(self.multipliers)
+            if torch.device(dev).type == "cuda":   # pinned and asynchronous: no host synchronisation in a forward
+                m = m.pin_memory().to(dev, non_blocking=True)
+            self._mult[dev] = m
+        return m
 
 
 class _CallSiteSums(object):
@@ -597,7 +653,6 @@ class _CallSiteSums(object):
         self.load = load
         self.acc = {}    # id -> (sums [G, n], scales [G, s], float64 device tensors, batches)
         self.meta = {}   # id -> (internal_name, what _tables needs of the call site, elements per group and batch)
-        self._mult_dev = {}
         self._loaded = None
 
     @property
@@ -605,13 +660,6 @@ class _CallSiteSums(object):
         return os.path.join(self.folder, self.FILE)
 
     # -- collect ---------------------------------------------------------------------------------------------------
-    def _device_multipliers(self, values, device, *key):
-        """``values`` as a float32 tensor on ``device``, made once per (device, ``key``)."""
-        mult = self._mult_dev.get((device,) + key)
-        if mult is None:
-            mult = self._mult_dev[(device,) + key] = torch.from_numpy(np.asarray(values, dtype=np.float32)).to(device)
-        return mult
-
     def _add(self, id, sums, scales, meta):
         prev = self.acc.get(id)
         if prev is None:
@@ -667,9 +715,10 @@ class _CallSiteSums(object):
 
 class ClipMseStatistics(_CallSiteSums):
     """Clipping-MSE curves (`collect_mse`): ``save_curve(t, tag, id, cfg)`` adds, per group of the quantizer ``cfg`` (a
-    ClipErrConfig, as collect_err passes) describes, the float64 sums of ops.clip_mse over ``multipliers`` (alpha = m * b
-    with prior "laplace", m * std with "gaus") and the group's b, std and width to device accumulators; ``__exit__``
-    writes clip_mse.pkl and curve.csv.  With ``load`` the instance reads clip_mse.pkl instead (on first use), for `-c mse`.
+    ClipErrConfig, as collect_err passes) describes, the float64 sums of its curve (``_curve``) over ``multipliers``
+    (alpha = m * b with prior "laplace", m * std with "gaus"; or the run's MseCandidates) and the group's b, std and width
+    to device accumulators; ``__exit__`` writes clip_mse.pkl and curve.csv.  With ``load`` the instance reads clip_mse.pkl
+    instead (on first use), for `-c mse`.
 
     curve.csv holds layer totals per element: mse = sum_g sum (x - q)^2 / sum_g count, and the reference's analytic
     curves (mse_analysis.py) per group at the same alpha, with that group's b or std and width (width + 1 for a positive
@@ -678,16 +727,13 @@ class ClipMseStatistics(_CallSiteSums):
     FLAG, USE, WHAT, GROUPS = "collect_mse", "-c mse", "clipping-MSE curve", "groups"
 
     def __init__(self, folder, multipliers=None, prior="laplace", base_dir=None, load=False):
-        self.multipliers = _mse_multipliers(multipliers, prior)
-        self.prior = prior
+        self.candidates = MseCandidates.of(multipliers, prior)
+        self.multipliers, self.prior = self.candidates.multipliers, self.candidates.prior
         super(ClipMseStatistics, self).__init__(folder, base_dir, load)
 
     # -- collect ---------------------------------------------------------------------------------------------------
     def save_curve(self, tensor, tag, id, cfg):
-        t, layout, cl, table = _stats_table(tensor.detach(), cfg, True)
-        sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive,
-                            self._device_multipliers(self.multipliers, t.device), prior=self.prior,
-                            bit_alloc=cfg.bit_alloc, solve_f64=not cfg.per_channel)
+        _, layout, _, table, sums = _curve(tensor.detach(), cfg, self.candidates)
         bits = table[:, 7] if cfg.bit_alloc else torch.full_like(table[:, 7], float(cfg.num_bits))
         self._add(id, sums, torch.stack([table[:, 3], table[:, 4], bits], 1).double(),
                   (tag, bool(cfg.positive), layout[0] * layout[2]))
@@ -774,14 +820,21 @@ def bit_candidates(rule, positive, num_bits):
     raise ValueError("bit allocation tables are measured under clipping %s, got %r" % (list(BIT_RULES[:3]), rule))
 
 
+@functools.lru_cache(maxsize=None)
+def _width_candidates(rule, positive, num_bits):
+    """The MseCandidates of ``bit_candidates(rule, positive, num_bits)``: constants, made once per key."""
+    return MseCandidates(*bit_candidates(rule, positive, num_bits))
+
+
 class BitMseStatistics(_CallSiteSums):
     """Per-channel error tables of bit allocation (`collect_bits`): ``save_table(t, tag, id, cfg)`` adds, for a call site
-    whose quantizer ``cfg`` (a ClipErrConfig) quantizes per channel with bit allocation, the float64 sums of one
-    ops.clip_mse launch over the 9 candidates of ``bit_candidates(rule, ...)`` and the channels' b and std to device
-    accumulators; other call sites are skipped.  Under rule "mse" (`-c mse`, the joint width-and-clip search) the launch is
-    one ops.clip_mse_grid over widths 0..8 times ``multipliers`` (alpha = m * b with ``prior`` "laplace", m * std with
-    "gaus"), and each width's error is the one at its best multiplier (``best_columns``).  ``__exit__`` writes bit_mse.pkl
-    and alloc.csv.  With ``load`` the instance reads bit_mse.pkl instead (on first use), for `-bap mse`."""
+    whose quantizer ``cfg`` (a ClipErrConfig) quantizes per channel with bit allocation, the float64 sums of its width
+    tables (``_width_tables``: one ops.clip_mse launch over the 9 candidates of ``bit_candidates(rule, ...)``) and the
+    channels' b and std to device accumulators; other call sites are skipped.  Under rule "mse" (`-c mse`, the joint
+    width-and-clip search) the launch is one ops.clip_mse_grid over widths 0..8 times ``multipliers`` (alpha = m * b with
+    ``prior`` "laplace", m * std with "gaus"; or the run's MseCandidates), and each width's error is the one at its best
+    multiplier (``best_columns``).  ``__exit__`` writes bit_mse.pkl and alloc.csv.  With ``load`` the instance reads
+    bit_mse.pkl instead (on first use), for `-bap mse`."""
     KIND, FILE, CSV = "bit_mse", "bit_mse.pkl", "alloc.csv"
     FLAG, USE, WHAT, GROUPS = "collect_bits", "-bap mse", "per-channel error table", "channels"
 
@@ -789,26 +842,17 @@ class BitMseStatistics(_CallSiteSums):
         if not load and rule not in BIT_RULES:
             raise ValueError("collect_bits measures under clipping %s, got %r" % (list(BIT_RULES), rule))
         self.rule = rule
+        self.candidates = None
         if rule == "mse":
-            self.multipliers = _mse_multipliers(multipliers, prior)
-            self.prior = prior
+            self.candidates = MseCandidates.of(multipliers, prior)
+            self.multipliers, self.prior = self.candidates.multipliers, self.candidates.prior
         super(BitMseStatistics, self).__init__(folder, base_dir, load)
 
     # -- collect ---------------------------------------------------------------------------------------------------
     def save_table(self, tensor, tag, id, cfg):
         if not (cfg.per_channel and cfg.bit_alloc):
             return
-        # an 8-bit table without allocation: every candidate brings its own width
-        t, layout, cl, table = _stats_table(tensor.detach(), cfg._replace(bit_alloc=False), True)
-        if self.rule == "mse":
-            sums = ops.clip_mse_grid(t, table, layout, cl, cfg.num_bits, cfg.positive,
-                                     self._device_multipliers(self.multipliers, t.device), range(9), prior=self.prior,
-                                     solve_f64=False)
-        else:
-            mults, prior = bit_candidates(self.rule, cfg.positive, cfg.num_bits)
-            sums = ops.clip_mse(t, table, layout, cl, cfg.num_bits, cfg.positive,
-                                self._device_multipliers(mults, t.device, bool(cfg.positive), cfg.num_bits), prior=prior,
-                                widths=range(9), solve_f64=False)
+        _, layout, _, table, sums = _width_tables(tensor.detach(), cfg, self.rule, self.candidates)
         self._add(id, sums, table[:, 3:5].double(), (tag, cfg, layout[0] * layout[2]))
 
     def _tables(self, groups):

@@ -377,3 +377,98 @@ def test_managers_launch_the_configured_candidates(monkeypatch, tmp_path, per_ch
             mults, p = bit_candidates(rule, True, 4)
             assert l["op"] == "clip_mse" and not l["bit_alloc"] and l["prior"] == p
             assert l["multipliers"] == torch.tensor(mults, dtype=torch.float32).tolist()
+
+
+@pytest.mark.parametrize("channels_last", [False, True], ids=["nchw", "cl"])
+@pytest.mark.parametrize("bits", [4, 8])
+@pytest.mark.parametrize("baa", [False, True])
+@pytest.mark.parametrize("positive", [False, True])
+@pytest.mark.parametrize("pcq", [False, True])
+def test_on_the_fly_routes_launch_what_collect_measures(monkeypatch, tmp_path, pcq, positive, baa, bits, channels_last):
+    """One call site, measured in collect mode (the manager's _clip_err) and on the fly (its quantizer): the
+    statistics-only launch and the candidate launch get the same arguments.  `-c mse -sm no` makes collect_mse's curve
+    with ops.clip_mse_select in place of ops.clip_mse; fly_bits makes collect_bits' width tables under each rule, with
+    want_params.  Collect runs -bap laplace: the prior fly_bits' -bap mse describes its call sites with."""
+    import inspect
+    import cnn_quantization_b200.manager as M
+    from cnn_quantization_b200 import ops
+    calls = []
+
+    def sums(a, k):
+        g = int(a["layout"][1])
+        s = torch.zeros(g, k + 1, dtype=torch.float64)
+        return (s, torch.zeros(g, k, 6)) if a.get("want_params") else s
+
+    results = {
+        "fused": lambda a: torch.zeros(int(a["layout"][1]), 12),
+        "clip_mse": lambda a: sums(a, len(a["multipliers"])),
+        "clip_mse_grid": lambda a: sums(a, 9 * len(a["multipliers"])),
+        "clip_mse_select": lambda a: (sums(a, len(a["multipliers"])), torch.zeros(int(a["layout"][1]), dtype=torch.int32),
+                                      torch.ones(3, int(a["layout"][1])), torch.ones(int(a["layout"][1]), 12)),
+    }
+
+    def recorder(name):
+        sig = inspect.signature(getattr(ops, name))
+
+        def rec(*args, **kw):
+            bound = sig.bind(*args, **kw)
+            bound.apply_defaults()
+            a = dict(bound.arguments)
+            a["nhwc"] = ops.nhwc(a.pop("x"))
+            table = a.pop("table", None)
+            if "multipliers" in a:
+                a["multipliers"] = torch.as_tensor(a["multipliers"]).tolist()
+            if a.get("widths") is not None:
+                a["widths"] = list(a["widths"])
+            res = results[name](a)
+            calls.append((name, a, table, res))
+            return res
+        return rec
+
+    for name in results:
+        monkeypatch.setattr(ops, name, recorder(name))
+    monkeypatch.setattr(ops, "allocate_select", lambda s, p, stats, target, multipliers=None, status=None: (
+        torch.full((s.shape[0],), 3.0), None, torch.ones(3, s.shape[0]), torch.ones(s.shape[0], 12)))
+    monkeypatch.setattr(ops, "quantize1", lambda x, *a, **kw: x)
+    x = torch.randn(2, 4, 4, 4)
+    if channels_last:
+        x = x.to(memory_format=torch.channels_last)
+    flags = dict(qtype="int%d" % bits, per_channel_quant_act=pcq, bit_alloc_act=baa, mse_multipliers=[1.0, 2.5, 4.0],
+                 mse_prior="gaus")
+
+    def run(collect, **over):
+        """[(op, arguments)] of the call site's measurement launches under a manager with ``flags`` and ``over``."""
+        args = M.make_args(**dict(flags, **over))
+        qm = M.QuantizationManagerInference(args, M.get_params(args))
+        del calls[:]
+        if collect:
+            qm._clip_err(x, "activation", "conv1_activation", positive, "conv1")
+        else:
+            q = qm.quantizers["activation"]
+            q.half_range = positive
+            q(x.clone(), "conv1_activation", "activation")
+        for i, (name, _, table, _) in enumerate(calls):   # each candidate launch reads the table of the launch before it
+            assert table is None if name == "fused" else table is calls[i - 1][3]
+        return [c[:2] for c in calls]
+
+    allocates = pcq and baa and bits == 4
+    fly_mse = run(False, clipping="mse", bit_alloc_prior="laplace")
+    assert [n for n, _ in fly_mse] == ["fused", "clip_mse_select"]
+    for rule in ("laplace", "gaus", "no", "mse"):
+        collect = run(True, clipping=rule, bit_alloc_prior="laplace", stats_mode="collect", stats_base_dir=str(tmp_path),
+                      collect_mse=True, collect_bits=pcq and baa)
+        (_, stats), (op, curve) = collect[:2]
+        assert op == "clip_mse" and stats["stats_only"] and stats["positive"] == positive
+        assert stats["layout"] == ((2, 4, 16) if pcq else (1, 1, 128)) and stats["channels_last"] == (pcq and channels_last)
+        assert curve["num_bits"] == bits and curve["bit_alloc"] == allocates and curve["multipliers"] == [1.0, 2.5, 4.0]
+        assert fly_mse[0][1] == stats
+        assert fly_mse[1][1] == {k: v for k, v in curve.items() if k not in ("want_params", "widths")}
+        tables = collect[2:]
+        if not allocates:
+            assert not tables
+            continue
+        fly_bits = run(False, clipping=rule, bit_alloc_prior="mse", fly_bits=True)
+        assert [n for n, _ in tables] == [n for n, _ in fly_bits] == ["fused", "clip_mse_grid" if rule == "mse" else "clip_mse"]
+        assert not tables[0][1]["bit_alloc"] and tables[1][1]["widths"] == list(range(9))
+        assert fly_bits[0][1] == tables[0][1]
+        assert fly_bits[1][1] == dict(tables[1][1], want_params=True)

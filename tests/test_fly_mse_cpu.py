@@ -149,7 +149,7 @@ def test_per_channel_route(record, baa):
     (f, fl, fk), (s, sl, sk), (a, al, ak) = record
     assert (f, s, a) == ("fused", "select", "apply")
     assert fl == sl == al == (2, 8, 9)
-    assert fk["stats_only"] and fk["positive"] and fk["num_bits"] == 4 and fk["bit_alloc"] == baa
+    assert fk["stats_only"] and fk["positive"] and fk["num_bits"] == (4 if baa else 8) and fk["bit_alloc"] == baa
     assert fk.get("bias") is None and ak["bias"] is None
     assert sk == dict(cl=False, num_bits=4, positive=True, prior="gaus", bit_alloc=baa, solve_f64=False, k=3)
     assert torch.equal(ak["delta"], torch.arange(8) + 1.0) and torch.equal(ak["offset"], -torch.arange(8) - 0.5)
@@ -190,3 +190,16 @@ def test_offline_refusals_unchanged():
     q.measure_entropy = True
     with pytest.raises(NotImplementedError, match=r"\(-me\)"):
         q(torch.zeros(2, 8, 3, 3), "conv1_activation", "activation")
+
+
+def test_bare_quantizer_refuses_bap_mse(record):
+    """`-baa -bap mse` without fly_bits: a per-channel call site refuses before any launch, as the ACIQ launch does; a
+    per-tensor one allocates nothing and runs."""
+    q = _quantizer(baa=True)
+    q.bit_alloc_prior = "mse"
+    with pytest.raises(NotImplementedError, match="needs -sm use"):
+        q(torch.randn(2, 8, 3, 3), "conv1_activation", "activation")
+    assert not record
+    q.pcq_a = False
+    q(torch.randn(2, 8, 3, 3), "conv1_activation", "activation")
+    assert [c[0] for c in record] == ["fused", "select", "apply"]
